@@ -7,6 +7,7 @@
  *   group_by_helper            crates/polars-mem-engine/src/executors/group_by.rs:60-98
  *   DataFrameJoinOps::_join_impl  crates/polars-ops/src/frame/join/mod.rs:125-459
  *   DataFrame::take_unchecked  crates/polars-core/src/frame/mod.rs:1238-1294
+ *   DataFrame::sort_impl       crates/polars-core/src/frame/mod.rs:1432-1561
  *   apply_operator             crates/polars-expr/src/expressions/binary.rs:61-131
  * (binding stubs: INTEGRATION.md).  Plain C: pointers, sizes, PODs.  No torch / C++ types.
  *
@@ -252,6 +253,23 @@ bl_status bl_join(const bl_column* left_key, const bl_column* right_key,
                   const bl_column* left_cols, int32_t n_left_cols, const bl_column* right_cols, int32_t n_right_cols,
                   int32_t how, int32_t nulls_equal, int32_t maintain_order, int32_t out_location,
                   bl_column* out_left_cols, bl_column* out_right_cols);
+
+/* ---- K9: sort  (DataFrame::sort_impl polars-core/src/frame/mod.rs:1432-1561; arg_sort_multiple arg_sort_multiple.rs:66-75) */
+enum { BL_SORT_DESCENDING = 1, BL_SORT_NULLS_LAST = 2 };
+/* The IdxSize permutation that sorts the rows by by[0], then by[1], ... (one chunk per column; any numeric dtype incl.
+ * 8/16-bit, and BL_BOOL: false < true).  flags[i]: bits above for by[i]; NULL = all ascending, nulls first
+ * (SortMultipleOptions, options.rs:85-105).  Values in the total order of reorder_cmp (polars-utils/src/sort.rs:113-128):
+ * floats by tot_cmp (NaN == NaN and greatest, -0.0 == +0.0), descending reverses it; null placement follows
+ * BL_SORT_NULLS_LAST only, and nulls compare equal.  The result is always the STABLE order (ties keep row order), which is
+ * the reference's answer wherever it pins one (single column: arg_sort.rs:118-185; maintain_order).
+ * limit >= 0 keeps the first `limit` rows of the sorted order (the (0, k) slice, frame/mod.rs:1482-1486).
+ * out_idx: BL_UINT32.  More than 2^32 - 1 rows, or a string key: BL_ERR_UNSUPPORTED. */
+bl_status bl_arg_sort(const bl_column* by, int32_t n_by, const int32_t* flags, int64_t limit,
+                      int32_t out_location, bl_column* out_idx);
+/* bl_arg_sort + one K4 gather of the payload columns (4- and 8-byte dtypes) at the first `limit` rows of the
+ * permutation: out_cols[i] = cols[i] in sorted order, validity included.  Key columns appear in cols if wanted. */
+bl_status bl_sort(const bl_column* by, int32_t n_by, const int32_t* flags, const bl_column* cols, int32_t n_cols,
+                  int64_t limit, int32_t out_location, bl_column* out_cols);
 
 /* ---- K6: radix hash partition (multi-GPU exchange step) --------------------------------- */
 /* partition id = hash_to_partition(dirty_hash(key), n_partitions)

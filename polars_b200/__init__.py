@@ -599,6 +599,51 @@ def join(left_key, right_key, left_cols: Sequence, right_cols: Sequence, how: st
     return _finish(list(lo)[:len(lc)], location), _finish(list(ro)[:len(rc)], location)
 
 
+SORT_DESCENDING, SORT_NULLS_LAST = 1, 2
+
+
+def _sort_flags(n_by: int, descending, nulls_last):
+    """bool (every column) or one bool per column -> BL_SORT_* words; a length mismatch raises as Polars does."""
+    def per_col(v, what):
+        if isinstance(v, (bool, np.bool_)):
+            return [bool(v)] * n_by
+        v = [bool(x) for x in v]
+        if len(v) != n_by:
+            raise ValueError(f"the length of `{what}` ({len(v)}) does not match the length of `by` ({n_by})")
+        return v
+    d, nl = per_col(descending, "descending"), per_col(nulls_last, "nulls_last")
+    return (C.c_int32 * n_by)(*[(SORT_DESCENDING if a else 0) | (SORT_NULLS_LAST if b else 0) for a, b in zip(d, nl)])
+
+
+def _sort_keys(by):
+    """one key column (array / Column / OutColumn / (values, valid)) or a list of them"""
+    return [_as_col(c) for c in by] if isinstance(by, list) else [_as_col(by)]
+
+
+def arg_sort(by, descending=False, nulls_last=False, limit: int | None = None, location: int = HOST):
+    """bl_arg_sort: the UInt32 permutation that sorts the rows by the key column(s) `by` (stable; see the header).
+    descending / nulls_last: a bool for every column or one bool per column.  limit: keep the first `limit` rows.
+    Host output: a numpy uint32 array; device output: an OutColumn."""
+    ks = _sort_keys(by)
+    arr, out = _col_array(ks), BlColumn()
+    _check(lib().bl_arg_sort(arr, C.c_int32(len(ks)), _sort_flags(len(ks), descending, nulls_last), C.c_int64(-1 if limit is None else int(limit)),
+                             C.c_int32(location), C.byref(out)))
+    res = _finish([out], location)[0]
+    return res[0] if location == HOST else res
+
+
+def sort(by, cols: Sequence, descending=False, nulls_last=False, limit: int | None = None, location: int = HOST):
+    """bl_sort: the payload columns `cols` (4- and 8-byte dtypes) in the order arg_sort(by, ...) gives, on the device.
+    Returns a list like `gather` returns."""
+    ks = _sort_keys(by)
+    cs = [_as_col(c) for c in cols]
+    karr = _col_array(ks)
+    carr, outs = (_col_array(cs) if cs else None), (BlColumn * max(len(cs), 1))()
+    _check(lib().bl_sort(karr, C.c_int32(len(ks)), _sort_flags(len(ks), descending, nulls_last), carr, C.c_int32(len(cs)),
+                         C.c_int64(-1 if limit is None else int(limit)), C.c_int32(location), outs))
+    return _finish(list(outs)[:len(cs)], location)
+
+
 def hash_partition(key, payload: Sequence, n_partitions: int, location: int = HOST):
     k = _as_col(key)
     ps = [_as_col(p) for p in payload]

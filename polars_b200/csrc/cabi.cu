@@ -346,6 +346,39 @@ bl_status bl_join(const bl_column* left_key, const bl_column* right_key, const b
     BL_CATCH
 }
 
+static void import_sort_keys(const bl_column* by, int32_t n_by, const int32_t* flags, std::vector<DevCol>& keys, std::vector<int>& fl) {
+    PLB_REQUIRE(by && n_by >= 1, BL_ERR_INVALID, "sort: no key column");
+    for (int i = 0; i < n_by; i++) {
+        PLB_REQUIRE(by[i].length == by[0].length, BL_ERR_INVALID, "sort: key columns differ in length");
+        keys.push_back(import_column(&by[i], 1));
+        fl.push_back(flags ? flags[i] : 0);
+    }
+}
+
+bl_status bl_arg_sort(const bl_column* by, int32_t n_by, const int32_t* flags, int64_t limit, int32_t out_location, bl_column* out_idx) {
+    BL_TRY
+    require_out(out_idx, "out_idx");
+    std::vector<DevCol> keys; std::vector<int> fl;
+    import_sort_keys(by, n_by, flags, keys, fl);
+    DevCol perm = op_arg_sort(keys, fl, limit);
+    export_column(perm, out_location, out_idx);
+    BL_CATCH
+}
+
+bl_status bl_sort(const bl_column* by, int32_t n_by, const int32_t* flags, const bl_column* cols, int32_t n_cols, int64_t limit, int32_t out_location, bl_column* out_cols) {
+    BL_TRY
+    PLB_REQUIRE(n_cols >= 0 && (n_cols == 0 || (cols && out_cols)), BL_ERR_INVALID, "sort: null payload / output");
+    std::vector<DevCol> keys, in, outs; std::vector<int> fl;
+    import_sort_keys(by, n_by, flags, keys, fl);
+    for (int i = 0; i < n_cols; i++) {
+        PLB_REQUIRE(cols[i].length == by[0].length, BL_ERR_INVALID, "sort: payload length differs from the keys");
+        in.push_back(import_column(&cols[i], 1));
+    }
+    op_sort(keys, fl, in, limit, outs);
+    if (!outs.empty()) export_many(outs, out_location, out_cols);
+    BL_CATCH
+}
+
 bl_status bl_hash_partition(const bl_column* key, const bl_column* payload, int32_t n_payload, int32_t n_partitions, int32_t out_location, bl_column* out_key,
                             bl_column* out_payload, int64_t* offsets) {
     BL_TRY

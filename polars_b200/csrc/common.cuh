@@ -165,6 +165,9 @@ DevPtr bitmap_slice(const uint32_t* bm, int64_t pos, int64_t len);      // bits 
 void exclusive_scan_u32_to_u64(const uint32_t* in, uint64_t* out, int64_t n, uint64_t* total_dev);
 void exclusive_scan_u64(const uint64_t* in, uint64_t* out, int64_t n, uint64_t* total_dev);
 void sort_pairs_u32(uint32_t* keys, uint32_t* vals, int64_t n, int key_bits = 32);   // stable LSD radix sort on the low key_bits, ascending (device)
+// multi-column arg_sort (sort.cu): flags[i] = BL_SORT_* of by[i]; the UInt32 permutation, truncated to limit (< 0: all rows)
+DevCol op_arg_sort(const std::vector<DevCol>& by, const std::vector<int>& flags, int64_t limit);
+void op_sort(const std::vector<DevCol>& by, const std::vector<int>& flags, const std::vector<DevCol>& cols, int64_t limit, std::vector<DevCol>& outs);
 void iota_u32(uint32_t* p, int64_t n, uint32_t base);
 inline int bits_for(uint64_t max_value) { int b = 1; while (b < 32 && (max_value >> b)) b++; return b; }   // digits the radix sort has to look at
 

@@ -206,32 +206,74 @@ void op_filter(const std::vector<DevCol>& cols, const DevCol& mask, std::vector<
     }
 }
 
-// ---------------------------------------------------------------------------- sort helper
-// Stable ascending LSD radix sort of (key u32, value u32) pairs, 8-bit digits — the ordering modes only
-// (maintain_order, ascending row lists of duplicate build keys, GroupsIdx), never the headline path.
-// Hand-written (round 1 called cub::DeviceRadixSort here).  Per pass:
-//   k_rs_hist     every CTA owns one contiguous chunk of the input; 256-bin shared-memory histogram -> hist[digit][cta]
-//   k_scan_u64    one exclusive scan over the digit-major matrix = global start of every (digit, cta) run
+// ---------------------------------------------------------------------------- radix sort
+// Stable ascending LSD radix sort of (key, u32 value) pairs, 8-bit digits, keys u32 or u64.  It serves the internal
+// ordering modes (maintain_order, ascending row lists of duplicate build keys, GroupsIdx: sort_pairs_u32) and the
+// public sort (sort.cu: one stage per encoded key column).  Per pass over digit `shift / 8`:
+//   k_rs_hist     every CTA owns one contiguous chunk of the input; 256-bin shared-memory histogram -> hist[digit][cta],
+//                 plus the digit's total over all CTAs (one atomic per CTA and digit)
+//   k_rs_scan     one CTA per digit: start of every (digit, cta) run = totals of the smaller digits + the exclusive scan
+//                 of the digit's row (the rows are independent, so the scan costs one launch instead of one long CTA)
 //   k_rs_scatter  the CTA walks its chunk tile by tile, in order.  Inside a tile warp w owns a contiguous segment and
 //                 ranks its items 32 at a time with __match_any_sync (lanes holding the same digit): rank = the warp's
 //                 running count of the digit + the number of equal-digit lanes below — original order is kept at every
-//                 level (tile, warp segment, round, lane), which is what makes the pass stable.
-// Only the digits below `key_bits` are processed (slot / row-index keys rarely need all 32 bits).
+//                 level (tile, warp segment, round, lane), which is what makes the pass stable.  The tile is then
+//                 staged in shared memory in digit order and every (tile, digit) run is written out contiguously, so
+//                 consecutive lanes store consecutive addresses (the K5r / K6 scatter design) instead of one sector each.
+// Only digits whose bits vary over the input are processed (`vary` = AND ^ OR of the keys, or the low key_bits).
 constexpr int RS_THREADS = 256, RS_ITEMS = 16, RS_TILE = RS_THREADS * RS_ITEMS, RS_WARPS = RS_THREADS / 32;
+constexpr int RS_MAX_CTAS = 1024;        // one k_rs_scan CTA covers a digit's row
 
-__global__ void __launch_bounds__(RS_THREADS) k_rs_hist(const uint32_t* __restrict__ keys, int64_t n, int64_t chunk, int shift, uint32_t* __restrict__ hist, int n_ctas) {
+template <typename K>
+__global__ void __launch_bounds__(RS_THREADS) k_rs_hist(const K* __restrict__ keys, int64_t n, int64_t chunk, int shift, uint32_t* __restrict__ hist, int n_ctas,
+                                                        uint32_t* __restrict__ digit_tot) {
     __shared__ unsigned h[256];
     h[threadIdx.x] = 0;
     __syncthreads();
     const int64_t lo = (int64_t)blockIdx.x * chunk, hi = min(n, lo + chunk);
-    for (int64_t i = lo + threadIdx.x; i < hi; i += RS_THREADS) atomicAdd(&h[(keys[i] >> shift) & 255u], 1u);
+    for (int64_t i = lo + threadIdx.x; i < hi; i += RS_THREADS) atomicAdd(&h[(unsigned)(keys[i] >> shift) & 255u], 1u);
     __syncthreads();
-    hist[(int64_t)threadIdx.x * n_ctas + blockIdx.x] = h[threadIdx.x];
+    const unsigned c = h[threadIdx.x];
+    hist[(int64_t)threadIdx.x * n_ctas + blockIdx.x] = c;
+    if (c) atomicAdd(&digit_tot[threadIdx.x], c);
 }
 
-__global__ void __launch_bounds__(RS_THREADS) k_rs_scatter(const uint32_t* __restrict__ keys_in, const uint32_t* __restrict__ vals_in, uint32_t* __restrict__ keys_out, uint32_t* __restrict__ vals_out,
+// grid = 256 (one CTA per digit), block = RS_MAX_CTAS
+__global__ void __launch_bounds__(RS_MAX_CTAS) k_rs_scan(const uint32_t* __restrict__ hist, const uint32_t* __restrict__ digit_tot, uint64_t* __restrict__ starts, int n_ctas) {
+    __shared__ uint64_t warp_sums[32];
+    const unsigned lane = lane_id(), warp = threadIdx.x >> 5, d = blockIdx.x;
+    // base of the digit = sum of the totals of the smaller digits (warps 0..7 hold digits 0..255)
+    uint64_t b = (threadIdx.x < d) ? digit_tot[threadIdx.x] : 0;
+    for (int o = 16; o; o >>= 1) b += __shfl_xor_sync(0xffffffffu, b, o);
+    if (lane == 0) warp_sums[warp] = b;
+    __syncthreads();
+    uint64_t base = 0;
+    for (int w = 0; w < RS_MAX_CTAS / 32; w++) base += warp_sums[w];
+    __syncthreads();
+    const uint64_t v = (int)threadIdx.x < n_ctas ? hist[(int64_t)d * n_ctas + threadIdx.x] : 0;
+    uint64_t x = v;
+    for (int o = 1; o < 32; o <<= 1) { uint64_t y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= (unsigned)o) x += y; }
+    if (lane == 31) warp_sums[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        uint64_t s = warp_sums[lane], t = s;
+        for (int o = 1; o < 32; o <<= 1) { uint64_t y = __shfl_up_sync(0xffffffffu, t, o); if (lane >= (unsigned)o) t += y; }
+        warp_sums[lane] = t - s;
+    }
+    __syncthreads();
+    if ((int)threadIdx.x < n_ctas) starts[(int64_t)d * n_ctas + threadIdx.x] = base + warp_sums[warp] + x - v;
+}
+
+// dynamic shared memory: RS_TILE keys followed by RS_TILE values
+template <typename K>
+__global__ void __launch_bounds__(RS_THREADS) k_rs_scatter(const K* __restrict__ keys_in, const uint32_t* __restrict__ vals_in, K* __restrict__ keys_out, uint32_t* __restrict__ vals_out,
                                                            int64_t n, int64_t chunk, int shift, const uint64_t* __restrict__ starts, int n_ctas) {
+    extern __shared__ __align__(16) unsigned char rs_smem[];
+    K* skey = reinterpret_cast<K*>(rs_smem);
+    uint32_t* sval = reinterpret_cast<uint32_t*>(skey + RS_TILE);
     __shared__ unsigned warp_cnt[RS_WARPS][256];
+    __shared__ unsigned dstart[256];            // tile-local start of each digit's run
+    __shared__ unsigned scan_w[RS_WARPS];
     __shared__ unsigned long long gbase[256];
     const unsigned lane = lane_id(), warp = threadIdx.x >> 5;
     gbase[threadIdx.x] = starts[(int64_t)threadIdx.x * n_ctas + blockIdx.x];
@@ -239,13 +281,13 @@ __global__ void __launch_bounds__(RS_THREADS) k_rs_scatter(const uint32_t* __res
     for (int64_t tile = lo; tile < hi; tile += RS_TILE) {
         for (int w = 0; w < RS_WARPS; w++) warp_cnt[w][threadIdx.x] = 0;
         __syncthreads();
-        uint32_t k[RS_ITEMS], v[RS_ITEMS]; unsigned rank[RS_ITEMS];
+        K k[RS_ITEMS]; uint32_t v[RS_ITEMS]; unsigned rank[RS_ITEMS];
 #pragma unroll
         for (int r = 0; r < RS_ITEMS; r++) {
             const int64_t i = tile + ((int64_t)warp * RS_ITEMS + r) * 32 + lane;
             const bool in = i < hi;
-            k[r] = in ? keys_in[i] : 0u; v[r] = in ? vals_in[i] : 0u;
-            const unsigned d = in ? ((k[r] >> shift) & 255u) : 256u;          // 256 = "no item": its own match class
+            k[r] = in ? keys_in[i] : K(0); v[r] = in ? vals_in[i] : 0u;
+            const unsigned d = in ? ((unsigned)(k[r] >> shift) & 255u) : 256u;     // 256 = "no item": its own match class
             const unsigned peers = __match_any_sync(0xffffffffu, d);
             const unsigned leader = __ffs(peers) - 1;
             unsigned old = 0;
@@ -255,48 +297,94 @@ __global__ void __launch_bounds__(RS_THREADS) k_rs_scatter(const uint32_t* __res
             __syncwarp();
         }
         __syncthreads();
-        // digit = threadIdx.x: exclusive scan of the warps' counts on top of the CTA's running global offset
-        {
-            unsigned long long run = gbase[threadIdx.x];
-            for (int w = 0; w < RS_WARPS; w++) { const unsigned c = warp_cnt[w][threadIdx.x]; warp_cnt[w][threadIdx.x] = (unsigned)(run - gbase[threadIdx.x]); run += c; }
-            __syncthreads();
-            // warp_cnt now holds offsets relative to the OLD gbase; publish the new base after everyone has read the old one below
+        // digit = threadIdx.x: the warps' exclusive offsets inside the digit's run, then the tile-local start of every run
+        unsigned tot = 0;
+        for (int w = 0; w < RS_WARPS; w++) { const unsigned c = warp_cnt[w][threadIdx.x]; warp_cnt[w][threadIdx.x] = tot; tot += c; }
+        unsigned x = tot;
+        for (int o = 1; o < 32; o <<= 1) { const unsigned y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= (unsigned)o) x += y; }
+        if (lane == 31) scan_w[warp] = x;
+        __syncthreads();
+        unsigned wbase = 0;
+        for (int w = 0; w < (int)warp; w++) wbase += scan_w[w];
+        dstart[threadIdx.x] = wbase + x - tot;
+        __syncthreads();
+        // stage the tile in digit order
 #pragma unroll
-            for (int r = 0; r < RS_ITEMS; r++) {
-                const int64_t i = tile + ((int64_t)warp * RS_ITEMS + r) * 32 + lane;
-                if (i < hi) {
-                    const unsigned d = (k[r] >> shift) & 255u;
-                    const unsigned long long pos = gbase[d] + warp_cnt[warp][d] + rank[r];
-                    keys_out[pos] = k[r]; vals_out[pos] = v[r];
-                }
+        for (int r = 0; r < RS_ITEMS; r++) {
+            const int64_t i = tile + ((int64_t)warp * RS_ITEMS + r) * 32 + lane;
+            if (i < hi) {
+                const unsigned d = (unsigned)(k[r] >> shift) & 255u;
+                const unsigned p = dstart[d] + warp_cnt[warp][d] + rank[r];
+                skey[p] = k[r]; sval[p] = v[r];
             }
-            __syncthreads();
-            gbase[threadIdx.x] = run;
         }
         __syncthreads();
+        // write every (tile, digit) run contiguously: staged position p of digit d goes to gbase[d] + (p - dstart[d])
+        const int cnt = (int)min((int64_t)RS_TILE, hi - tile);
+#pragma unroll 4
+        for (int p = threadIdx.x; p < cnt; p += RS_THREADS) {
+            const K kk = skey[p];
+            const unsigned d = (unsigned)(kk >> shift) & 255u;
+            const unsigned long long pos = gbase[d] + (unsigned)(p - dstart[d]);
+            keys_out[pos] = kk; vals_out[pos] = sval[p];
+        }
+        __syncthreads();
+        gbase[threadIdx.x] += tot;
     }
+}
+
+template <typename K>
+static bool radix_sort_pairs(K* k0, uint32_t* v0, K* k1, uint32_t* v1, int64_t n, uint64_t vary, int* passes_run) {
+    int digits[8], passes = 0;
+    for (int d = 0; d < (int)sizeof(K); d++) if ((vary >> (8 * d)) & 255u) digits[passes++] = d;
+    if (passes_run) *passes_run = n > 1 ? passes : 0;
+    if (n <= 1 || passes == 0) return false;
+    PLB_REQUIRE(n <= (int64_t)0xFFFFFFFFll, BL_ERR_UNSUPPORTED, "radix sort: more than 2^32 - 1 rows");
+    Context& c = ctx();
+    const size_t smem = (size_t)RS_TILE * (sizeof(K) + 4);
+    static bool attr_set = false;        // serialised by the context lock
+    if (!attr_set) {
+        PLB_CUDA(cudaFuncSetAttribute(k_rs_scatter<uint32_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(RS_TILE * 8)));
+        PLB_CUDA(cudaFuncSetAttribute(k_rs_scatter<uint64_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(RS_TILE * 12)));
+        attr_set = true;
+    }
+    int per_sm = 0;
+    PLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_rs_scatter<K>, RS_THREADS, smem));
+    const int64_t tiles = (n + RS_TILE - 1) / RS_TILE;
+    const int n_ctas0 = (int)std::min<int64_t>(tiles, std::min<int64_t>((int64_t)c.sm_count * std::max(per_sm, 1), RS_MAX_CTAS));
+    const int64_t chunk = (tiles + n_ctas0 - 1) / n_ctas0 * RS_TILE;
+    const int n_ctas = (int)((n + chunk - 1) / chunk);       // no empty trailing CTA
+    DevPtr hist = dev_alloc((size_t)256 * n_ctas * 4), starts = dev_alloc((size_t)256 * n_ctas * 8), tot = dev_alloc((size_t)passes * 256 * 4);
+    dev_memset(tot->p, 0, (size_t)passes * 256 * 4);
+    K *ki = k0, *ko = k1;
+    uint32_t *vi = v0, *vo = v1;
+    for (int p = 0; p < passes; p++) {
+        const int shift = 8 * digits[p];
+        uint32_t* dt = as<uint32_t>(tot) + 256 * p;
+        PLB_LAUNCH("sort_hist", k_rs_hist<K>, n_ctas, RS_THREADS, 0, ki, n, chunk, shift, as<uint32_t>(hist), n_ctas, dt);
+        PLB_LAUNCH("sort_scan", k_rs_scan, 256, RS_MAX_CTAS, 0, as<uint32_t>(hist), dt, as<uint64_t>(starts), n_ctas);
+        PLB_LAUNCH("sort_scatter", k_rs_scatter<K>, n_ctas, RS_THREADS, smem, ki, vi, ko, vo, n, chunk, shift, as<uint64_t>(starts), n_ctas);
+        std::swap(ki, ko); std::swap(vi, vo);
+    }
+    return ki != k0;
+}
+
+bool radix_sort_pairs_u32(uint32_t* k0, uint32_t* v0, uint32_t* k1, uint32_t* v1, int64_t n, uint64_t vary, int* passes_run) {
+    return radix_sort_pairs<uint32_t>(k0, v0, k1, v1, n, vary, passes_run);
+}
+bool radix_sort_pairs_u64(uint64_t* k0, uint32_t* v0, uint64_t* k1, uint32_t* v1, int64_t n, uint64_t vary, int* passes_run) {
+    return radix_sort_pairs<uint64_t>(k0, v0, k1, v1, n, vary, passes_run);
 }
 
 void sort_pairs_u32(uint32_t* keys, uint32_t* vals, int64_t n, int key_bits) {
     if (n <= 1) return;
     if (key_bits < 1 || key_bits > 32) key_bits = 32;
-    Context& c = ctx();
     const int passes = (key_bits + 7) / 8;
-    const int64_t tiles = (n + RS_TILE - 1) / RS_TILE;
-    const int n_ctas = (int)std::min<int64_t>(tiles, (int64_t)c.sm_count * 2);      // the (digit x cta) matrix is scanned by one CTA: keep it small
-    const int64_t chunk = (tiles + n_ctas - 1) / n_ctas * RS_TILE;
+    const uint64_t digits = passes == 4 ? 0xFFFFFFFFull : ((1ull << (8 * passes)) - 1);
     DevPtr k2 = dev_alloc((size_t)n * 4), v2 = dev_alloc((size_t)n * 4);
-    DevPtr hist = dev_alloc((size_t)256 * n_ctas * 4), starts = dev_alloc((size_t)256 * n_ctas * 8);
-    uint32_t *ki = keys, *vi = vals, *ko = as<uint32_t>(k2), *vo = as<uint32_t>(v2);
-    for (int p = 0; p < passes; p++) {
-        PLB_LAUNCH("sort_hist", k_rs_hist, n_ctas, RS_THREADS, 0, ki, n, chunk, 8 * p, as<uint32_t>(hist), n_ctas);
-        exclusive_scan_u32_to_u64(as<uint32_t>(hist), as<uint64_t>(starts), (int64_t)256 * n_ctas, nullptr);
-        PLB_LAUNCH("sort_scatter", k_rs_scatter, n_ctas, RS_THREADS, 0, ki, vi, ko, vo, n, chunk, 8 * p, as<uint64_t>(starts), n_ctas);
-        std::swap(ki, ko); std::swap(vi, vo);
-    }
-    if (ki != keys) {
-        PLB_CUDA(cudaMemcpyAsync(keys, ki, (size_t)n * 4, cudaMemcpyDeviceToDevice, c.stream));
-        PLB_CUDA(cudaMemcpyAsync(vals, vi, (size_t)n * 4, cudaMemcpyDeviceToDevice, c.stream));
+    if (radix_sort_pairs<uint32_t>(keys, vals, as<uint32_t>(k2), as<uint32_t>(v2), n, digits, nullptr)) {
+        PLB_CUDA(cudaMemcpyAsync(keys, k2->p, (size_t)n * 4, cudaMemcpyDeviceToDevice, ctx().stream));
+        PLB_CUDA(cudaMemcpyAsync(vals, v2->p, (size_t)n * 4, cudaMemcpyDeviceToDevice, ctx().stream));
     }
 }
 

@@ -139,20 +139,21 @@ static void release_inputs(SeriesExport* inputs, size_t n) {
     }
 }
 
-enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN };
+enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT };
 
 // ---- kwargs ----------------------------------------------------------------------------------------
 // register_plugin_function(kwargs={...}) pickles the dict (py-polars/src/polars/plugins.py:100-115) and the caller hands
 // the bytes through (plugin.rs:70-137; Rust plugins read them with serde-pickle).  The subset a flat {str: bool | int |
 // float | str | None} dict produces under protocols 2..5 is parsed here: PROTO FRAME EMPTY_DICT MARK (SHORT_)BINUNICODE
 // BININT BININT1 BININT2 LONG1 BINFLOAT NEWTRUE NEWFALSE NONE MEMOIZE BINPUT SETITEM SETITEMS STOP.
-struct Kwargs { std::vector<std::pair<std::string, double>> num; std::vector<std::pair<std::string, std::string>> str;
+struct Kwargs { std::vector<std::pair<std::string, double>> num; std::vector<std::pair<std::string, std::string>> str; std::vector<std::string> bools;
     double get(const char* k, double dflt) const { for (auto& e : num) if (e.first == k) return e.second; return dflt; }
+    bool is_bool(const char* k) const { for (auto& e : bools) if (e == k) return true; return false; }
     std::string gets(const char* k, const char* dflt) const { for (auto& e : str) if (e.first == k) return e.second; return dflt; } };
 static Kwargs parse_kwargs(const uint8_t* p, size_t n) {
     Kwargs kw;
     if (!p || n == 0) return kw;
-    struct Val { int kind; double num; std::string s; };      // kind: 0 none, 1 number, 2 string, 3 dict marker, 4 mark
+    struct Val { int kind; double num; std::string s; };      // kind: 0 none, 1 number, 2 string, 3 dict marker, 4 mark, 5 bool
     std::vector<Val> st;
     size_t i = 0;
     auto need = [&](size_t k) { PLB_REQUIRE(i + k <= n, BL_ERR_INVALID, "plugin kwargs: truncated pickle"); };
@@ -160,7 +161,8 @@ static Kwargs parse_kwargs(const uint8_t* p, size_t n) {
         for (size_t j = from; j + 1 < st.size(); j += 2) {
             PLB_REQUIRE(st[j].kind == 2, BL_ERR_UNSUPPORTED, "plugin kwargs: only string keys are supported");
             if (st[j + 1].kind == 2) kw.str.push_back({st[j].s, st[j + 1].s});
-            else kw.num.push_back({st[j].s, st[j + 1].kind == 1 ? st[j + 1].num : 0.0});
+            else kw.num.push_back({st[j].s, (st[j + 1].kind == 1 || st[j + 1].kind == 5) ? st[j + 1].num : 0.0});
+            if (st[j + 1].kind == 5) kw.bools.push_back(st[j].s);
         }
         st.resize(from);
     };
@@ -182,8 +184,8 @@ static Kwargs parse_kwargs(const uint8_t* p, size_t n) {
             case 0x8a: { need(1); const size_t l = p[i++]; need(l); int64_t v = 0; for (size_t b = 0; b < l && b < 8; b++) v |= (int64_t)p[i + b] << (8 * b);
                          if (l > 0 && l < 8 && (p[i + l - 1] & 0x80)) v |= -((int64_t)1 << (8 * l)); st.push_back({1, (double)v, ""}); i += l; break; }  // LONG1
             case 'G': { need(8); uint64_t b = 0; for (int k = 0; k < 8; k++) b = (b << 8) | p[i + k]; double d; memcpy(&d, &b, 8); st.push_back({1, d, ""}); i += 8; break; }   // BINFLOAT (big endian)
-            case 0x88: st.push_back({1, 1.0, ""}); break;                        // NEWTRUE
-            case 0x89: st.push_back({1, 0.0, ""}); break;                        // NEWFALSE
+            case 0x88: st.push_back({5, 1.0, ""}); break;                        // NEWTRUE
+            case 0x89: st.push_back({5, 0.0, ""}); break;                        // NEWFALSE
             case 'N': st.push_back({0, 0, ""}); break;                           // NONE
             case 's': { PLB_REQUIRE(st.size() >= 3, BL_ERR_INVALID, "plugin kwargs: malformed pickle"); flush_items(st.size() - 2); break; }       // SETITEM
             case 'u': { size_t m = st.size(); while (m > 0 && st[m - 1].kind != 4) m--; PLB_REQUIRE(m > 0, BL_ERR_INVALID, "plugin kwargs: malformed pickle");
@@ -200,7 +202,7 @@ static int join_how_of(int op) { return op; }
 static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, const Kwargs& kw, SeriesExport* ret) {
     std::lock_guard<std::recursive_mutex> lk(ctx().mu);
     PLB_REQUIRE(n >= 1, BL_ERR_INVALID, "plugin: no input series");
-    if (kind != P_GROUP && kind != P_JOIN) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
+    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
     std::vector<std::vector<bl_column>> chunks(n);
     std::vector<DevCol> in;
     for (size_t i = 0; i < n; i++) { int dt; chunks[i] = input_chunks(inputs[i], &dt); in.push_back(import_column(chunks[i].data(), (int)chunks[i].size())); }
@@ -228,6 +230,20 @@ static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, co
             bl_column h; export_column(o, BL_HOST, &h);
             fill_array(array, h);
             fill_schema(schema, name, format_of(o.dtype));
+        } else if (kind == P_SORT) {
+            // inputs: the `by` columns -> UInt32 permutation.  kwargs descending / nulls_last: a bool (every column) or an int
+            // bitmask (bit i = column i)
+            std::vector<int> flags(n, 0);
+            for (size_t j = 0; j < n; j++) {
+                for (auto f : {std::make_pair("descending", (int)BL_SORT_DESCENDING), std::make_pair("nulls_last", (int)BL_SORT_NULLS_LAST)}) {
+                    const int64_t v = (int64_t)kw.get(f.first, 0);
+                    if (kw.is_bool(f.first) ? v != 0 : j < 63 && ((v >> j) & 1)) flags[j] |= f.second;
+                }
+            }
+            DevCol perm = op_arg_sort(in, flags, -1);
+            bl_column h; export_column(perm, BL_HOST, &h);
+            fill_array(array, h);
+            fill_schema(schema, name, format_of(BL_UINT32));
         } else if (kind == P_GROUP) {
             // inputs: key_0 .. key_{k-1}, value (LEN: keys only)  ->  struct {key, key_1, ..., agg}, groups in first-occurrence order
             const bool is_len = op == BL_AGG_LEN;
@@ -305,6 +321,7 @@ static void field_entry(PluginOp kind, int op, const ArrowSchema* fields, size_t
     switch (kind) {
         case P_ARITH: fill_schema(out, name, format_of((op == BL_OP_TRUE_DIV && dt >= 0 && dt <= BL_UINT64) ? BL_FLOAT64 : (dt < 0 ? BL_INT64 : dt))); break;
         case P_CMP: fill_schema(out, name, "b"); break;
+        case P_SORT: fill_schema(out, name, format_of(BL_UINT32)); break;
         case P_FILTER: case P_GATHER: fill_schema(out, name, format_of(dt < 0 ? BL_INT64 : dt)); break;
         case P_GROUP: {
             const size_t nk = op == BL_AGG_LEN ? n : (n > 0 ? n - 1 : 0);
@@ -368,4 +385,5 @@ PLUGIN(join_left_idx, P_JOIN, BL_JOIN_LEFT)
 PLUGIN(join_full_idx, P_JOIN, BL_JOIN_FULL)
 PLUGIN(join_semi_idx, P_JOIN, BL_JOIN_SEMI)
 PLUGIN(join_anti_idx, P_JOIN, BL_JOIN_ANTI)
+PLUGIN(arg_sort, P_SORT, 0)                     /* kwargs: descending, nulls_last (bool or bitmask); inputs = by columns */
 }

@@ -20,6 +20,8 @@ Recognised:
   * GroupBy(keys=[col, ...], aggs ⊆ {col.sum/mean/min/max/count/first/last/var/std/n_unique, len}) over a DataFrameScan, optionally through
     one Filter(col <cmp> literal)                      -> bl_filter_cmp + bl_groupby_agg / bl_groupby_agg_keys
   * Join(inner|left|semi|anti, one key column per side) of two DataFrameScans -> bl_hash_join + bl_gather
+  * Sort(by=[col, ...] of numeric / Boolean columns, slice None or (0, k)) of a DataFrameScan -> bl_arg_sort (limit = k)
+    + bl_gather of the numeric columns (other columns: Polars' take of the same permutation)
 """
 from __future__ import annotations
 
@@ -231,6 +233,82 @@ def _plan_join(plb, nt, root_id, node):
     return run
 
 
+def _host_column(series):
+    """pl.Series -> (values, valid | None) numpy arrays with null slots filled (Boolean included)."""
+    if series.null_count() == 0:
+        return series.to_numpy(), None
+    fill = False if str(series.dtype) == "Boolean" else 0
+    return series.fill_null(fill).to_numpy(), ~series.is_null().to_numpy()
+
+
+_SORTABLE = set(_NUMERIC) | {"Int8", "Int16", "UInt8", "UInt16", "Boolean"}
+
+
+def _sort_slice_limit(slc):
+    """Sort.slice = None | (offset, len, id) (visitor/nodes.rs:246-257, 533-549): offset 0 becomes the limit."""
+    if slc is None:
+        return None
+    if not isinstance(slc, (tuple, list)) or len(slc) not in (2, 3) or (len(slc) == 3 and slc[2] is not None):
+        raise _Unsupported("sort slice")
+    offset, length = slc[0], slc[1]
+    if not isinstance(offset, int) or not isinstance(length, int) or offset != 0 or length < 0:
+        raise _Unsupported("sort slice with a nonzero offset")
+    return length
+
+
+def _plan_sort(plb, nt, root_id, node):
+    """Sort(input=DataFrameScan, by_column=[Column, ...], sort_options=(maintain_order, nulls_last, descending), slice).
+    The library's sort is always stable, which is what maintain_order asks for and a valid order when it is not set.
+    Key dtypes are checked here, on the Sort node's schema (NodeTraverser.get_schema, visit.rs:127-131): a key the device
+    cannot order (String, temporal, nested ...) leaves the node to Polars.  Every column of the frame is materialised:
+    the 4- and 8-byte numeric ones with K4 on the device, any other column with Polars' own take of the same permutation."""
+    opts, by_column = getattr(node, "sort_options", None), getattr(node, "by_column", None)
+    if not isinstance(opts, (tuple, list)) or len(opts) != 3 or not isinstance(by_column, (tuple, list)):
+        raise _Unsupported("sort options")
+    _maintain_order, nulls_last, descending = opts
+    by = [_column_name(nt, e.node) for e in by_column]
+    if not by:
+        raise _Unsupported("sort without keys")
+    nulls_last, descending = list(nulls_last), list(descending)
+    # Polars broadcasts a single flag to every key (SortMultipleOptions)
+    if len(nulls_last) == 1:
+        nulls_last *= len(by)
+    if len(descending) == 1:
+        descending *= len(by)
+    if len(nulls_last) != len(by) or len(descending) != len(by):
+        raise _Unsupported("sort flags")
+    limit = _sort_slice_limit(getattr(node, "slice", None))
+    if not hasattr(nt, "get_schema"):
+        raise _Unsupported("no schema to check the sort keys against")
+    schema = {str(k): str(v) for k, v in dict(nt.get_schema()).items()}
+    for c in by:
+        if schema.get(c) not in _SORTABLE:
+            raise _Unsupported(f"sort key {c}: dtype {schema.get(c)}")
+    frame = _scan_frame(nt, node.input)
+    nt.set_node(root_id)
+
+    def run(*_args: Any, **_kwargs: Any):
+        import polars as pl
+        df = frame().rechunk()
+        dev_cols = [c for c in df.columns if str(df.schema[c]) in _NUMERIC]          # K4 takes 4- and 8-byte elements
+        idx = plb.arg_sort([_host_column(df.get_column(c)) for c in by], descending=descending, nulls_last=nulls_last, limit=limit,
+                           location=plb.DEVICE)
+        res = {}
+        if dev_cols:
+            outs = plb.gather([_host_column(df.get_column(c)) for c in dev_cols], idx.view(), check_bounds=False)
+            for c, (v, m) in zip(dev_cols, outs):
+                s = pl.Series(c, v)
+                res[c] = s.set(pl.Series(~m), None) if m is not None else s
+        rest = [c for c in df.columns if c not in res]
+        if rest:
+            taken = df.select(rest)[pl.Series(idx.to_numpy()[0])]
+            for c in rest:
+                res[c] = taken.get_column(c)
+        return pl.DataFrame([res[c] for c in df.columns])
+
+    return run
+
+
 def execute_with_b200(nt: Any, duration_since_start: int | None = None, *, raise_on_fail: bool = False) -> None:
     """The post-optimisation callback.  Leaves the plan untouched when the root is not a supported shape."""
     import polars_b200 as plb
@@ -242,6 +320,8 @@ def execute_with_b200(nt: Any, duration_since_start: int | None = None, *, raise
             fn = _plan_group_by(plb, nt, root_id, root)
         elif kind == "Join":
             fn = _plan_join(plb, nt, root_id, root)
+        elif kind == "Sort":
+            fn = _plan_sort(plb, nt, root_id, root)
         else:
             raise _Unsupported(kind)
         nt.set_udf(fn)
