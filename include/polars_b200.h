@@ -148,7 +148,21 @@ enum { BL_AGG_SUM = 0, BL_AGG_MEAN = 1, BL_AGG_MIN = 2, BL_AGG_MAX = 3, BL_AGG_C
        /* evaluated per group over the reference's GroupsIdx (row lists in row order), not by the fused atomics path: */
        BL_AGG_FIRST = 6, BL_AGG_LAST = 7,   /* value at the group's first / last row, nulls included (dispatch.rs:57-120) */
        BL_AGG_VAR = 8, BL_AGG_STD = 9,      /* Welford in row order, f64; null when count <= ddof (aggregations/mod.rs:1020-1178, take_agg/var.rs:11-41) */
-       BL_AGG_N_UNIQUE = 10 };              /* distinct values per group, a null counts as one (aggregations/dispatch.rs:285-345); UInt32; bl_groupby_agg only */
+       BL_AGG_N_UNIQUE = 10,                /* distinct values per group, a null counts as one (aggregations/dispatch.rs:285-345); UInt32; bl_groupby_agg only */
+       BL_AGG_MEDIAN = 11,                  /* quantile(0.5, LINEAR) (aggregations/mod.rs:385-408) */
+       BL_AGG_QUANTILE = 12 };              /* probability and method from bl_agg_param: bl_groupby_agg_params only (aggregations/mod.rs:297-383) */
+/* Interpolation of BL_AGG_QUANTILE (QuantileMethod, polars-compute/src/rolling/mod.rs:40-48; Polars' default is NEAREST).
+ * Per group with m valid values and c nulls (quantile.rs:21-65): float_idx = (m - 1) * q + c into the values sorted nulls first
+ * in the total order (NaN greatest, -0.0 == +0.0); NEAREST takes round(float_idx) (half away from zero), LOWER / MIDPOINT /
+ * LINEAR trunc(float_idx), HIGHER ceil(float_idx), EQUIPROBABLE max(ceil(m * q) - 1, 0) + c; MIDPOINT and LINEAR interpolate
+ * towards the next value in f64 when float_idx is not whole.  A group without a valid value gives null. */
+enum { BL_QUANTILE_NEAREST = 0, BL_QUANTILE_LOWER = 1, BL_QUANTILE_HIGHER = 2, BL_QUANTILE_MIDPOINT = 3, BL_QUANTILE_LINEAR = 4,
+       BL_QUANTILE_EQUIPROBABLE = 5 };
+typedef struct bl_agg_param {
+    double quantile;        /* in [0, 1]; NaN or outside: BL_ERR_UNSUPPORTED (the reference returns an all-null column of the input dtype) */
+    int32_t method;         /* BL_QUANTILE_* */
+    int32_t reserved;
+} bl_agg_param;
 /* delta degrees of freedom of VAR / STD travel in bits 16..23 of `kind` (Polars' default is 1) */
 #define BL_AGG_WITH_DDOF(kind, ddof) ((kind) | ((ddof) << 16))
 typedef struct bl_agg {
@@ -162,8 +176,10 @@ typedef struct bl_agg {
  * out_key = key taken at each group's first row (group_by/mod.rs:258-266).
  * Output dtypes: SUM keeps the dtype (Int8/16,UInt8/16 -> Int64), ints wrap; MEAN -> FLOAT64
  * (FLOAT32 stays); MIN/MAX keep dtype; COUNT/LEN -> UINT32.  All-null group: SUM 0, MEAN/MIN/MAX null.
- * FIRST/LAST keep dtype; VAR/STD -> FLOAT64 (FLOAT32 stays).  A call that asks for any of FIRST/LAST/VAR/STD is evaluated
- * whole over GroupsIdx (groups then come in first-occurrence order), like bl_set_deterministic. */
+ * FIRST/LAST keep dtype; VAR/STD/MEDIAN/QUANTILE -> FLOAT64 (FLOAT32 stays).  A call that asks for any of
+ * FIRST/LAST/VAR/STD/MEDIAN/QUANTILE is evaluated whole over GroupsIdx (groups then come in first-occurrence order), like
+ * bl_set_deterministic.  MEDIAN / QUANTILE on a BL_BOOL column: BL_ERR_UNSUPPORTED; BL_AGG_QUANTILE needs
+ * bl_groupby_agg_params (here: BL_ERR_INVALID).  All MEDIAN / QUANTILE aggregations of one value column share one sort. */
 bl_status bl_groupby_agg(const bl_column* key_chunks, int32_t n_key_chunks, const bl_agg* aggs, int32_t n_aggs,
                          int32_t maintain_order, int32_t out_location, bl_column* out_key, bl_column* out_aggs);
 
@@ -173,6 +189,11 @@ bl_status bl_groupby_agg(const bl_column* key_chunks, int32_t n_key_chunks, cons
  * -0 == +0, NaN == NaN).  out_keys[i] = keys[i] taken at each group's first row; the rest as bl_groupby_agg. */
 bl_status bl_groupby_agg_keys(const bl_column* keys, int32_t n_keys, const bl_agg* aggs, int32_t n_aggs,
                               int32_t maintain_order, int32_t out_location, bl_column* out_keys, bl_column* out_aggs);
+/* bl_groupby_agg_keys with per-aggregation parameters: params[i] is read only where aggs[i].kind == BL_AGG_QUANTILE
+ * (params may be NULL when there is none).  bl_groupby_agg_keys is this call with params = NULL.  An unknown method, or a
+ * BL_AGG_QUANTILE without params: BL_ERR_INVALID. */
+bl_status bl_groupby_agg_params(const bl_column* keys, int32_t n_keys, const bl_agg* aggs, const bl_agg_param* params, int32_t n_aggs,
+                                int32_t maintain_order, int32_t out_location, bl_column* out_keys, bl_column* out_aggs);
 
 /* Group tuples: the reference's GroupsIdx{first, all} (polars-core/src/frame/group_by/position.rs:16-22)
  * as built by group_by_threaded_slice with sorted = true (hashing.rs:116-167, finish_group_order :41-63),
@@ -287,7 +308,8 @@ typedef struct bl_groupby bl_groupby;
  * track_first != 0 records each group's first row index (one extra 32-bit atomic per row); it is
  * required for bl_groupby_finish(maintain_order != 0). */
 /* value_nullable[i] == 0 promises that aggregation i's column never carries nulls (saves its null
- * counter: smaller table entries); NULL = every column may be nullable. */
+ * counter: smaller table entries); NULL = every column may be nullable.  MEDIAN / QUANTILE cannot be pre-aggregated:
+ * BL_ERR_UNSUPPORTED here and in bl_groupby_agg_partitioned. */
 bl_status bl_groupby_create(int32_t key_dtype, const int32_t* agg_kinds, const int32_t* value_dtypes, const int32_t* value_nullable,
                             int32_t n_aggs, int64_t expected_groups, int32_t track_first, bl_groupby** out);
 /* Accumulate one batch: key + one value column per agg (values[i] ignored for LEN).  Columns may

@@ -26,13 +26,33 @@ NP_OF = {v: k for k, v in DTYPES.items()}
 BOOL = 10
 OPS = {"add": 0, "sub": 1, "mul": 2, "floordiv": 3, "mod": 4, "truediv": 5}
 CMPS = {"eq": 0, "ne": 1, "lt": 2, "le": 3, "gt": 4, "ge": 5}
-AGGS = {"sum": 0, "mean": 1, "min": 2, "max": 3, "count": 4, "len": 5, "first": 6, "last": 7, "var": 8 | (1 << 16), "std": 9 | (1 << 16), "n_unique": 10}
+AGGS = {"sum": 0, "mean": 1, "min": 2, "max": 3, "count": 4, "len": 5, "first": 6, "last": 7, "var": 8 | (1 << 16), "std": 9 | (1 << 16), "n_unique": 10,
+        "median": 11}
+QUANTILE = 12
+QUANTILE_METHODS = {"nearest": 0, "lower": 1, "higher": 2, "midpoint": 3, "linear": 4, "equiprobable": 5}
 
 
 def _agg_kind(kind: str) -> int:
-    """"var" / "std" default to ddof = 1 (Polars); "var:0", "std:2" ... carry an explicit ddof (BL_AGG_WITH_DDOF)."""
+    """"var" / "std" default to ddof = 1 (Polars); "var:0", "std:2" ... carry an explicit ddof (BL_AGG_WITH_DDOF).
+    "quantile:<q>[:<method>]" is BL_AGG_QUANTILE; its parameters come from _agg_param."""
     name, _, dd = kind.partition(":")
+    if name == "quantile":
+        return QUANTILE
     return (AGGS[name] & 0xFFFF) | (int(dd) << 16) if dd else AGGS[name]
+
+
+def _agg_param(kind: str) -> tuple[float, int] | None:
+    """"quantile:<q>" (method nearest, Polars' default) or "quantile:<q>:<method>" -> (q, BL_QUANTILE_*); None for other kinds."""
+    name, _, rest = kind.partition(":")
+    if name != "quantile":
+        return None
+    q, _, method = rest.partition(":")
+    if not q:
+        raise ValueError(f"{kind!r}: a quantile is written 'quantile:<q>' or 'quantile:<q>:<method>'")
+    method = method or "nearest"
+    if method not in QUANTILE_METHODS:
+        raise ValueError(f"{kind!r}: unknown quantile method {method!r} (one of {', '.join(QUANTILE_METHODS)})")
+    return float(q), QUANTILE_METHODS[method]
 JOINS = {"inner": 0, "left": 1, "semi": 2, "anti": 3, "full": 4}
 ORDERS = {"none": 0, "left": 1, "left_right": 2, "right": 3, "right_left": 4}
 STATUS = {1: "INVALID", 2: "CUDA", 3: "OOM", 4: "UNSUPPORTED", 5: "DTYPE", 6: "BOUNDS"}
@@ -50,6 +70,10 @@ class BlStringColumn(C.Structure):
 
 class BlAgg(C.Structure):
     _fields_ = [("kind", C.c_int32), ("n_chunks", C.c_int32), ("values", C.POINTER(BlColumn))]
+
+
+class BlAggParam(C.Structure):
+    _fields_ = [("quantile", C.c_double), ("method", C.c_int32), ("reserved", C.c_int32)]
 
 
 class B200Error(RuntimeError):
@@ -526,7 +550,8 @@ def group_by_agg_partitioned(key, aggs: Sequence, my_rank: int, peer_halves: Seq
 
 
 def group_by_agg_keys(keys: Sequence, aggs: Sequence, maintain_order: bool = False, location: int = HOST):
-    """Several key columns (one chunk each); aggs as in group_by_agg.  Returns ([key_outs], [agg_outs])."""
+    """Several key columns (one chunk each); aggs as in group_by_agg, plus "quantile:<q>[:<method>]" (bl_groupby_agg_params).
+    Returns ([key_outs], [agg_outs])."""
     kcols = [_as_col(c) for c in keys]
     karr = _col_array(kcols)
     keep, agg_structs = [], []
@@ -544,8 +569,14 @@ def group_by_agg_keys(keys: Sequence, aggs: Sequence, maintain_order: bool = Fal
         agg_structs.append(BlAgg(_agg_kind(kind), len(chunks), C.cast(arr, C.POINTER(BlColumn))))
     aarr = (BlAgg * max(len(agg_structs), 1))(*agg_structs)
     out_keys, out_aggs = (BlColumn * len(kcols))(), (BlColumn * max(len(agg_structs), 1))()
-    _check(lib().bl_groupby_agg_keys(karr, C.c_int32(len(kcols)), aarr, C.c_int32(len(agg_structs)), C.c_int32(int(maintain_order)), C.c_int32(location),
-                                     out_keys, out_aggs))
+    params = [_agg_param(kind) for kind, _ in aggs]
+    if any(p is not None for p in params):
+        parr = (BlAggParam * len(params))(*[BlAggParam(*(p or (0.0, 0)), 0) for p in params])
+        _check(lib().bl_groupby_agg_params(karr, C.c_int32(len(kcols)), aarr, parr, C.c_int32(len(agg_structs)), C.c_int32(int(maintain_order)),
+                                           C.c_int32(location), out_keys, out_aggs))
+    else:
+        _check(lib().bl_groupby_agg_keys(karr, C.c_int32(len(kcols)), aarr, C.c_int32(len(agg_structs)), C.c_int32(int(maintain_order)), C.c_int32(location),
+                                         out_keys, out_aggs))
     res = _finish(list(out_keys) + list(out_aggs)[: len(agg_structs)], location)
     return res[: len(kcols)], res[len(kcols):]
 

@@ -202,6 +202,11 @@ bl_status bl_groupby_agg(const bl_column* key_chunks, int32_t n_key_chunks, cons
 
 bl_status bl_groupby_agg_keys(const bl_column* keys, int32_t n_keys, const bl_agg* aggs, int32_t n_aggs, int32_t maintain_order, int32_t out_location,
                               bl_column* out_keys, bl_column* out_aggs) {
+    return bl_groupby_agg_params(keys, n_keys, aggs, nullptr, n_aggs, maintain_order, out_location, out_keys, out_aggs);
+}
+
+bl_status bl_groupby_agg_params(const bl_column* keys, int32_t n_keys, const bl_agg* aggs, const bl_agg_param* params, int32_t n_aggs, int32_t maintain_order,
+                                int32_t out_location, bl_column* out_keys, bl_column* out_aggs) {
     BL_TRY
     PLB_REQUIRE(keys && n_keys >= 1 && out_keys, BL_ERR_INVALID, "groupby_agg_keys: null keys / output");
     PLB_REQUIRE(n_aggs == 0 || (aggs && out_aggs), BL_ERR_INVALID, "groupby_agg_keys: null aggs / outputs");
@@ -234,7 +239,7 @@ bl_status bl_groupby_agg_keys(const bl_column* keys, int32_t n_keys, const bl_ag
     DevCol ok, first; std::vector<DevCol> oa;
     bool needs_groups_idx = ctx().deterministic;
     for (int i = 0; i < n_aggs; i++) needs_groups_idx |= (aggs[i].kind & 0xFFFF) >= BL_AGG_FIRST;
-    if (needs_groups_idx) op_group_by_exact(packed, kinds, vptr, first, oa);
+    if (needs_groups_idx) op_group_by_exact(packed, kinds, vptr, first, oa, params);
     else {
         GroupByState st(BL_UINT64, kinds, dts, nullable, 0, true);
         st.consume_all(packed, vptr);

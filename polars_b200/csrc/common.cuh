@@ -158,7 +158,12 @@ DevCol op_group_first_ids(const DevCol& key);
 DevCol op_pack_keys(const std::vector<DevCol>& keys);
 void op_group_tuples(const DevCol& key, DevCol& out_first, DevCol& out_offsets, DevCol& out_all);
 // deterministic mode: GroupsIdx + one sequential fold per group in the reference's order (groupby_exact.cu)
-void op_group_by_exact(const DevCol& key, const std::vector<int>& kinds, const std::vector<const DevCol*>& values, DevCol& out_first, std::vector<DevCol>& outs);
+// params[i] (quantile, method) is read where kinds[i] == BL_AGG_QUANTILE; nullptr = none given
+void op_group_by_exact(const DevCol& key, const std::vector<int>& kinds, const std::vector<const DevCol*>& values, DevCol& out_first, std::vector<DevCol>& outs,
+                       const bl_agg_param* params = nullptr);
+// per-group quantiles over GroupsIdx (offsets: G + 1 entries, all: row lists; quantile.cu): outs[k] = quantile qs[k] with methods[k]
+void op_group_quantiles(const DevCol& offsets, const DevCol& all, const DevCol& values, const std::vector<double>& qs, const std::vector<int>& methods,
+                        std::vector<DevCol>& outs);
 DevPtr bitmap_and(const uint32_t* a, const uint32_t* b, const uint32_t* c, int64_t bits);
 int64_t bitmap_popcount(const uint32_t* bm, int64_t bits);
 DevPtr bitmap_slice(const uint32_t* bm, int64_t pos, int64_t len);      // bits [pos, pos + len) as a fresh word-aligned bitmap

@@ -1109,6 +1109,7 @@ GroupByState::GroupByState(int key_dt, const std::vector<int>& kinds, const std:
             case BL_AGG_MAX: ap.main = add_word(flt ? W_MAX_F64 : (sgn ? W_MAX_S64 : W_MAX_U64)); ap.nullcnt = null_word(); ap.out_dtype = ap.in_dtype; L.need_len = 1; break;
             case BL_AGG_COUNT: ap.nullcnt = null_word(); ap.out_dtype = BL_UINT32; L.need_len = 1; break;
             case BL_AGG_LEN: ap.out_dtype = BL_UINT32; L.need_len = 1; break;
+            case BL_AGG_MEDIAN: case BL_AGG_QUANTILE: fail(BL_ERR_UNSUPPORTED, "group_by: median / quantile cannot be pre-aggregated (use bl_groupby_agg)");
             default: fail(BL_ERR_INVALID, "group_by: unknown aggregation kind");
         }
         plans.push_back(ap);

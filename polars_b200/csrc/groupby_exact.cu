@@ -140,11 +140,27 @@ static int exact_out_dtype(int kind, int in_dtype) {
 }
 
 // key: the (single, possibly packed) key column; values[i] == nullptr for LEN.  Groups come in first-occurrence order.
-void op_group_by_exact(const DevCol& key, const std::vector<int>& kinds, const std::vector<const DevCol*>& values, DevCol& out_first, std::vector<DevCol>& outs) {
+// MEDIAN / QUANTILE go to op_group_quantiles (quantile.cu), one call per distinct value column.
+void op_group_by_exact(const DevCol& key, const std::vector<int>& kinds, const std::vector<const DevCol*>& values, DevCol& out_first, std::vector<DevCol>& outs,
+                       const bl_agg_param* params) {
+    std::vector<double> qs(kinds.size(), 0.5);
+    std::vector<int> methods(kinds.size(), BL_QUANTILE_LINEAR);      // MEDIAN = quantile(0.5, Linear) (aggregations/mod.rs:385-408)
+    for (size_t i = 0; i < kinds.size(); i++) {      // argument errors before any device work
+        const int kind = kinds[i] & 0xFFFF;
+        PLB_REQUIRE(kind >= BL_AGG_SUM && kind <= BL_AGG_QUANTILE && kind != BL_AGG_N_UNIQUE, BL_ERR_INVALID, "group_by: unknown aggregation kind");
+        if (kind != BL_AGG_QUANTILE) continue;
+        PLB_REQUIRE(params != nullptr, BL_ERR_INVALID, "group_by: BL_AGG_QUANTILE needs its parameters (bl_groupby_agg_params)");
+        PLB_REQUIRE(params[i].method >= BL_QUANTILE_NEAREST && params[i].method <= BL_QUANTILE_EQUIPROBABLE, BL_ERR_INVALID,
+                    "group_by: unknown quantile method " + std::to_string(params[i].method));
+        // the reference answers an all-null column of the input dtype (aggregations/mod.rs:309-312): the caller's CPU path
+        PLB_REQUIRE(params[i].quantile >= 0.0 && params[i].quantile <= 1.0, BL_ERR_UNSUPPORTED, "group_by: quantile " + std::to_string(params[i].quantile) + " is outside [0, 1]");
+        qs[i] = params[i].quantile; methods[i] = params[i].method;
+    }
     DevCol offsets, all;
     op_group_tuples(key, out_first, offsets, all);
     const int64_t G = out_first.len;
-    outs.clear();
+    outs.assign(kinds.size(), DevCol());
+    std::vector<bool> done(kinds.size(), false);
     for (size_t i = 0; i < kinds.size(); i++) {
         const int kind = kinds[i] & 0xFFFF, ddof = (kinds[i] >> 16) & 0xFF;
         const DevCol* v = values[i];
@@ -152,7 +168,21 @@ void op_group_by_exact(const DevCol& key, const std::vector<int>& kinds, const s
         const int in_dt = v ? v->dtype : BL_INT64;
         PLB_REQUIRE(kind == BL_AGG_LEN || in_dt == BL_INT64 || in_dt == BL_UINT64 || in_dt == BL_INT32 || in_dt == BL_UINT32 || in_dt == BL_FLOAT64 || in_dt == BL_FLOAT32, BL_ERR_UNSUPPORTED,
                     std::string("group_by: value dtype ") + dtype_name(in_dt) + " is outside the hot path");
-        PLB_REQUIRE(kind >= BL_AGG_SUM && kind <= BL_AGG_STD, BL_ERR_INVALID, "group_by: unknown aggregation kind");
+        if (done[i]) continue;
+        if (kind == BL_AGG_MEDIAN || kind == BL_AGG_QUANTILE) {      // every median / quantile of this value column: one sort
+            std::vector<size_t> at;
+            std::vector<double> q; std::vector<int> m;
+            for (size_t j = i; j < kinds.size(); j++) {
+                const int kj = kinds[j] & 0xFFFF;
+                if ((kj == BL_AGG_MEDIAN || kj == BL_AGG_QUANTILE) && values[j]->values == v->values && values[j]->validity == v->validity && values[j]->dtype == v->dtype) {
+                    at.push_back(j); q.push_back(qs[j]); m.push_back(methods[j]); done[j] = true;
+                }
+            }
+            std::vector<DevCol> qo;
+            op_group_quantiles(offsets, all, *v, q, m, qo);
+            for (size_t k = 0; k < at.size(); k++) outs[at[k]] = qo[k];
+            continue;
+        }
         const bool nullable = kind == BL_AGG_MEAN || kind == BL_AGG_MIN || kind == BL_AGG_MAX || kind >= BL_AGG_FIRST;
         DevCol o = make_col(exact_out_dtype(kind, in_dt), G, nullable);
         if (G > 0) {
@@ -169,7 +199,7 @@ void op_group_by_exact(const DevCol& key, const std::vector<int>& kinds, const s
                 default: PLB_LAUNCH("k5x_fold_groups", k_seg_agg<float>, grid, 128, 0, a); break;
             }
         }
-        outs.push_back(o);
+        outs[i] = o;
     }
 }
 

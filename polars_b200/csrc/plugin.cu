@@ -11,6 +11,7 @@
 // Ownership (plugin.rs:118-125): the caller forgets the inputs, so this side releases every input
 // array and every input SeriesExport; the return value carries its own release callbacks.
 // Errors: `ret` is left untouched (private_data == NULL) and the message is kept thread-local.
+#include <cmath>
 #include <cstdlib>
 #include <string>
 #include <vector>
@@ -251,6 +252,18 @@ static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, co
             const size_t nk = is_len ? n : n - 1;
             int agg_kind = op;
             if (op == BL_AGG_VAR || op == BL_AGG_STD) agg_kind = BL_AGG_WITH_DDOF(op, (int)kw.get("ddof", 1));
+            bl_agg_param qp{0.5, BL_QUANTILE_LINEAR, 0};
+            if (op == BL_AGG_QUANTILE) {      // kwargs: quantile (float, required), method (str, default "nearest")
+                qp.quantile = kw.get("quantile", std::nan(""));
+                PLB_REQUIRE(!std::isnan(qp.quantile), BL_ERR_INVALID, "plugin group_quantile: the `quantile` kwarg is required");
+                const std::string m = kw.gets("method", "nearest");
+                static const char* names[] = {"nearest", "lower", "higher", "midpoint", "linear", "equiprobable"};
+                qp.method = -1;
+                for (int j = 0; j < 6; j++) if (m == names[j]) qp.method = j;
+                PLB_REQUIRE(qp.method >= 0, BL_ERR_INVALID, "plugin group_quantile: unknown method '" + m + "'");
+            }
+            // median / quantile are Float64 for every integer width: 8/16-bit columns aggregate as Int64, as in bl_groupby_agg
+            if ((op == BL_AGG_MEDIAN || op == BL_AGG_QUANTILE) && dtype_is_small_int(in[n - 1].dtype)) in[n - 1] = op_cast_small_int(in[n - 1], BL_INT64, false);
             std::vector<DevCol> key_outs; DevCol agg_out;
             if (nk == 1 && op <= BL_AGG_LEN && !ctx().deterministic) {
                 const DevCol& a = in[0];
@@ -260,11 +273,11 @@ static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, co
                 DevCol ok; std::vector<DevCol> oa;
                 st.finish(true, &a, ok, oa);
                 key_outs.push_back(ok); agg_out = oa[0];
-            } else {      // several key columns, first / last / var / std, deterministic mode: GroupsIdx + sequential folds
+            } else {      // several key columns, first / last / var / std / median / quantile, deterministic mode: GroupsIdx
                 std::vector<DevCol> keys(in.begin(), in.begin() + nk);
                 DevCol packed = nk == 1 ? keys[0] : op_pack_keys(keys);
                 DevCol first; std::vector<DevCol> oa;
-                op_group_by_exact(packed, {agg_kind}, {is_len ? nullptr : &in[n - 1]}, first, oa);
+                op_group_by_exact(packed, {agg_kind}, {is_len ? nullptr : &in[n - 1]}, first, oa, &qp);
                 for (auto& k : keys) { std::vector<DevCol> o; op_gather({k}, first, false, o); key_outs.push_back(o[0]); }
                 agg_out = oa[0];
             }
@@ -328,7 +341,7 @@ static void field_entry(PluginOp kind, int op, const ArrowSchema* fields, size_t
             const int v = (op == BL_AGG_LEN || n < 2) ? -1 : dtype_from_format(fields[n - 1].format);
             int adt = v < 0 ? BL_INT64 : v;
             if (v == BL_INT8 || v == BL_INT16 || v == BL_UINT8 || v == BL_UINT16) adt = (op == BL_AGG_SUM) ? BL_INT64 : v;
-            if (op == BL_AGG_MEAN || op == BL_AGG_VAR || op == BL_AGG_STD) adt = v == BL_FLOAT32 ? BL_FLOAT32 : BL_FLOAT64;
+            if (op == BL_AGG_MEAN || op == BL_AGG_VAR || op == BL_AGG_STD || op == BL_AGG_MEDIAN || op == BL_AGG_QUANTILE) adt = v == BL_FLOAT32 ? BL_FLOAT32 : BL_FLOAT64;
             if (op == BL_AGG_COUNT || op == BL_AGG_LEN) adt = BL_UINT32;
             std::vector<std::pair<std::string, int>> kids;
             for (size_t j = 0; j < nk; j++) { const int kd = dtype_from_format(fields[j].format); kids.push_back({j == 0 ? "key" : "key_" + std::to_string(j), kd < 0 ? BL_INT64 : kd}); }
@@ -380,6 +393,8 @@ PLUGIN(group_first, P_GROUP, BL_AGG_FIRST)
 PLUGIN(group_last, P_GROUP, BL_AGG_LAST)
 PLUGIN(group_var, P_GROUP, BL_AGG_VAR)          /* kwargs: ddof (default 1) */
 PLUGIN(group_std, P_GROUP, BL_AGG_STD)
+PLUGIN(group_median, P_GROUP, BL_AGG_MEDIAN)
+PLUGIN(group_quantile, P_GROUP, BL_AGG_QUANTILE)    /* kwargs: quantile (float, required), method (str, default "nearest") */
 PLUGIN(join_inner_idx, P_JOIN, BL_JOIN_INNER)   /* kwargs: nulls_equal; 2k inputs = k key columns per side */
 PLUGIN(join_left_idx, P_JOIN, BL_JOIN_LEFT)
 PLUGIN(join_full_idx, P_JOIN, BL_JOIN_FULL)
