@@ -284,13 +284,31 @@ enum { BL_SORT_DESCENDING = 1, BL_SORT_NULLS_LAST = 2 };
  * BL_SORT_NULLS_LAST only, and nulls compare equal.  The result is always the STABLE order (ties keep row order), which is
  * the reference's answer wherever it pins one (single column: arg_sort.rs:118-185; maintain_order).
  * limit >= 0 keeps the first `limit` rows of the sorted order (the (0, k) slice, frame/mod.rs:1482-1486).
- * out_idx: BL_UINT32.  More than 2^32 - 1 rows, or a string key: BL_ERR_UNSUPPORTED. */
+ * out_idx: BL_UINT32.  More than 2^32 - 1 rows: BL_ERR_UNSUPPORTED.  String / binary keys: bl_arg_sort_keys. */
 bl_status bl_arg_sort(const bl_column* by, int32_t n_by, const int32_t* flags, int64_t limit,
                       int32_t out_location, bl_column* out_idx);
 /* bl_arg_sort + one K4 gather of the payload columns (4- and 8-byte dtypes) at the first `limit` rows of the
  * permutation: out_cols[i] = cols[i] in sorted order, validity included.  Key columns appear in cols if wanted. */
 bl_status bl_sort(const bl_column* by, int32_t n_by, const int32_t* flags, const bl_column* cols, int32_t n_cols,
                   int64_t limit, int32_t out_location, bl_column* out_cols);
+
+/* Dense lexicographic rank (RankMethod::Dense, rank.rs:61-188) of a LargeUtf8 / LargeBinary column: UInt32, 1-based, bytes
+ * compared unsigned with a proper prefix first; descending != 0 ranks the largest value 1; null rows give null.
+ * *n_distinct (optional) = number of distinct non-null values = the largest rank.  More than 2^32 - 2 rows: BL_ERR_UNSUPPORTED. */
+bl_status bl_string_rank(const bl_string_column* chunks, int32_t n_chunks, int32_t descending, int32_t out_location,
+                         bl_column* out_rank, int64_t* n_distinct);
+
+typedef struct bl_sort_key {
+    const bl_column* column;          /* numeric / Boolean key (one chunk), or NULL */
+    const bl_string_column* strings;  /* LargeUtf8 / LargeBinary key, or NULL; exactly one of the two is set */
+    int32_t n_chunks;                 /* chunks of `strings` */
+    int32_t flags;                    /* BL_SORT_DESCENDING | BL_SORT_NULLS_LAST */
+} bl_sort_key;
+/* bl_arg_sort over keys that may be strings: each string key is ranked (bl_string_rank, ascending) and sorted as that
+ * UInt32 column with its own flags; everything else exactly as bl_arg_sort.  A descriptor with both or neither pointer set,
+ * or keys of different lengths: BL_ERR_INVALID.  String payload columns are materialised with bl_string_gather on the
+ * permutation, numeric ones with bl_gather. */
+bl_status bl_arg_sort_keys(const bl_sort_key* by, int32_t n_by, int64_t limit, int32_t out_location, bl_column* out_idx);
 
 /* ---- K6: radix hash partition (multi-GPU exchange step) --------------------------------- */
 /* partition id = hash_to_partition(dirty_hash(key), n_partitions)

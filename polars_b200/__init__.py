@@ -76,6 +76,10 @@ class BlAggParam(C.Structure):
     _fields_ = [("quantile", C.c_double), ("method", C.c_int32), ("reserved", C.c_int32)]
 
 
+class BlSortKey(C.Structure):
+    _fields_ = [("column", C.POINTER(BlColumn)), ("strings", C.POINTER(BlStringColumn)), ("n_chunks", C.c_int32), ("flags", C.c_int32)]
+
+
 class B200Error(RuntimeError):
     def __init__(self, status: int, msg: str):
         super().__init__(f"[{STATUS.get(status, status)}] {msg}")
@@ -365,8 +369,53 @@ class StringColumn:
                               None if self.bits is None else self.bits.ctypes.data, None)
 
 
-def _str_array(cols: Sequence[StringColumn]):
+class DeviceStringColumn:
+    """A library-owned device copy of a string column (bl_string_column_to with BL_DEVICE; chunks are concatenated).
+    Every string entry point takes it wherever it takes a StringColumn.  Freed on `.free()` / garbage collection."""
+
+    def __init__(self, col=None, *, st: BlStringColumn | None = None):
+        """col: a StringColumn or a list of chunks, copied to the device; st: a library-owned device output to wrap"""
+        if st is None:
+            chunks = col if isinstance(col, list) else [col]
+            st = BlStringColumn()
+            _check(lib().bl_string_column_to(_str_array(chunks), C.c_int32(len(chunks)), C.c_int32(DEVICE), C.byref(st)))
+        self.st = st
+        self.length = int(self.st.length)
+
+    def struct(self) -> BlStringColumn:
+        return self.st
+
+    def free(self):
+        if self.st.owner:
+            lib().bl_string_column_free.restype = None
+            lib().bl_string_column_free(C.byref(self.st))
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+def _str_array(cols: Sequence):
     return (BlStringColumn * len(cols))(*[c.struct() for c in cols])
+
+
+def _is_string_key(x) -> bool:
+    """a string column, or a list of string chunks"""
+    if isinstance(x, list):
+        return bool(x) and all(isinstance(c, (StringColumn, DeviceStringColumn)) for c in x)
+    return isinstance(x, (StringColumn, DeviceStringColumn))
+
+
+def string_rank(col, descending: bool = False, location: int = HOST):
+    """bl_string_rank: -> ((ranks, valid) | OutColumn, n_distinct).  Dense 1-based UInt32 rank in unsigned byte order
+    (a proper prefix first); descending ranks the largest value 1; null rows are null."""
+    chunks = col if isinstance(col, list) else [col]
+    arr = _str_array(chunks)
+    out, nd = BlColumn(), C.c_int64()
+    _check(lib().bl_string_rank(arr, C.c_int32(len(chunks)), C.c_int32(int(descending)), C.c_int32(location), C.byref(out), C.byref(nd)))
+    return _finish([out], location)[0], int(nd.value)
 
 
 def string_encode(col, location: int = HOST):
@@ -394,15 +443,15 @@ def _string_out_to_list(out: BlStringColumn) -> list:
         lib().bl_string_column_free(C.byref(out))
 
 
-def string_gather(col, idx) -> list:
-    """bl_string_gather with host output: -> list of bytes / None."""
+def string_gather(col, idx, location: int = HOST):
+    """bl_string_gather: -> list of bytes / None (host output) or a DeviceStringColumn (device output)."""
     chunks = col if isinstance(col, list) else [col]
     arr = _str_array(chunks)
     ic = _as_col(idx)
     ist = ic.struct()
     out = BlStringColumn()
-    _check(lib().bl_string_gather(arr, C.c_int32(len(chunks)), C.byref(ist), C.c_int32(HOST), C.byref(out)))
-    return _string_out_to_list(out)
+    _check(lib().bl_string_gather(arr, C.c_int32(len(chunks)), C.byref(ist), C.c_int32(location), C.byref(out)))
+    return _string_out_to_list(out) if location == HOST else DeviceStringColumn(st=out)
 
 
 def group_by_agg_strings(key, aggs: Sequence, maintain_order: bool = False):
@@ -651,10 +700,39 @@ def _sort_keys(by):
     return [_as_col(c) for c in by] if isinstance(by, list) else [_as_col(by)]
 
 
+def _has_string_key(by) -> bool:
+    return any(_is_string_key(k) for k in by) if isinstance(by, list) else _is_string_key(by)
+
+
+def _arg_sort_keys(by, descending, nulls_last, limit, location):
+    """bl_arg_sort_keys: `by` holds numeric keys and string keys (a StringColumn / DeviceStringColumn, or a list of chunks)"""
+    keys = by if isinstance(by, list) else [by]
+    flags = _sort_flags(len(keys), descending, nulls_last)
+    descs, keep = (BlSortKey * len(keys))(), []
+    for i, k in enumerate(keys):
+        if _is_string_key(k):
+            chunks = k if isinstance(k, list) else [k]
+            arr = _str_array(chunks)
+            keep.append(arr)
+            descs[i] = BlSortKey(None, C.cast(arr, C.POINTER(BlStringColumn)), len(chunks), flags[i])
+        else:
+            c = _as_col(k)
+            st = c.struct()
+            keep.append((c, st))
+            descs[i] = BlSortKey(C.pointer(st), None, 0, flags[i])
+    out = BlColumn()
+    _check(lib().bl_arg_sort_keys(descs, C.c_int32(len(keys)), C.c_int64(-1 if limit is None else int(limit)), C.c_int32(location), C.byref(out)))
+    return _finish([out], location)[0]
+
+
 def arg_sort(by, descending=False, nulls_last=False, limit: int | None = None, location: int = HOST):
     """bl_arg_sort: the UInt32 permutation that sorts the rows by the key column(s) `by` (stable; see the header).
     descending / nulls_last: a bool for every column or one bool per column.  limit: keep the first `limit` rows.
+    A key may be a string column (StringColumn / DeviceStringColumn, or a list of its chunks): then bl_arg_sort_keys.
     Host output: a numpy uint32 array; device output: an OutColumn."""
+    if _has_string_key(by):
+        res = _arg_sort_keys(by, descending, nulls_last, limit, location)
+        return res[0] if location == HOST else res
     ks = _sort_keys(by)
     arr, out = _col_array(ks), BlColumn()
     _check(lib().bl_arg_sort(arr, C.c_int32(len(ks)), _sort_flags(len(ks), descending, nulls_last), C.c_int64(-1 if limit is None else int(limit)),
@@ -665,7 +743,11 @@ def arg_sort(by, descending=False, nulls_last=False, limit: int | None = None, l
 
 def sort(by, cols: Sequence, descending=False, nulls_last=False, limit: int | None = None, location: int = HOST):
     """bl_sort: the payload columns `cols` (4- and 8-byte dtypes) in the order arg_sort(by, ...) gives, on the device.
-    Returns a list like `gather` returns."""
+    With a string key: bl_arg_sort_keys on the device, then bl_gather of the payload (string payloads: string_gather of
+    the permutation).  Returns a list like `gather` returns."""
+    if _has_string_key(by):
+        perm = _arg_sort_keys(by, descending, nulls_last, limit, DEVICE)
+        return gather(cols, perm, check_bounds=False, location=location) if len(cols) else []
     ks = _sort_keys(by)
     cs = [_as_col(c) for c in cols]
     karr = _col_array(ks)

@@ -24,18 +24,9 @@
 
 #include "common.cuh"
 #include "dev_utils.cuh"
+#include "strings.cuh"
 
 namespace plb {
-
-struct DevStr {
-    int64_t len = 0, data_bytes = 0, null_count = 0;
-    DevPtr offsets;    // (len + 1) x int64, offsets[0] == 0
-    DevPtr data;       // data_bytes
-    DevPtr validity;   // word-padded bitmap or null
-    const int64_t* off() const { return as<int64_t>(offsets); }
-    const uint8_t* bytes() const { return as<uint8_t>(data); }
-    const uint32_t* vm() const { return validity ? as<uint32_t>(validity) : nullptr; }
-};
 
 __device__ __forceinline__ uint64_t str_mix(uint64_t h, uint64_t w) { h = (h ^ w) * 0xff51afd7ed558ccdULL; return h ^ (h >> 29); }
 __device__ __forceinline__ uint64_t str_hash_bytes(const uint8_t* __restrict__ p, int64_t n, uint64_t seed) {
