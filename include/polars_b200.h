@@ -310,6 +310,36 @@ typedef struct bl_sort_key {
  * permutation, numeric ones with bl_gather. */
 bl_status bl_arg_sort_keys(const bl_sort_key* by, int32_t n_by, int64_t limit, int32_t out_location, bl_column* out_idx);
 
+/* ---- asof join  (_join_asof_dispatch polars-ops/src/frame/join/asof/mod.rs:325-394; by keys groups.rs:39-345) ------- */
+enum { BL_ASOF_BACKWARD = 0, BL_ASOF_FORWARD = 1, BL_ASOF_NEAREST = 2 };
+/* The reference's take_idx: out_right_idx (BL_UINT32, left_on->length rows, nullable; a null slot holds BL_IDX_NULL) names,
+ * per left row, the right row its asof search picks.  The frame is then left ‖ right.take(idx) (_finish_join, mod.rs:300-321).
+ * Precondition, checked on the device on every call with at least one left row (per group when n_by > 0; an empty left side
+ * returns an empty index at once, which is the reference's answer whatever the right side holds): the non-null left `on` values are
+ * non-decreasing (nulls anywhere), the right `on` column is nulls first and then non-decreasing (is_sorted with the default
+ * SortOptions), both in the total order (NaN greatest, -0.0 == +0.0).  Outside it: BL_ERR_UNSUPPORTED, the message naming
+ * the side; the caller's CPU path gives the reference's answer there.  Inside it, the reference's cursors (mod.rs:47-200)
+ * give, per non-null left value l over V = [z, n), the right's non-null rows (a null l, or an empty V, gives null):
+ *   BL_ASOF_BACKWARD  the last j in V with r_j <= l (r_j < l when allow_eq == 0), total order
+ *   BL_ASOF_FORWARD   the first j in V with r_j >= l (r_j > l when allow_eq == 0), total order
+ *   BL_ASOF_NEAREST   partial order (the reference compares with >, >= and ==, mod.rs:143-180): U = the first j in V with
+ *                     r_j > l, else n; with allow_eq, U > z and r_{U-1} == l: U - 1.  Otherwise U moves to the last row of its
+ *                     run of equal values (U < n), L = (the first j in [z, U) with r_j >= l) - 1, or U - 1 when there is none;
+ *                     the one of L (>= z) and U (< n) that exists, and with both U when |l - r_U| <= |l - r_L|, else L.
+ * tolerance (NULL, or a non-null length-1 column of the key dtype; for an 8/16-bit key also Int32, the type the reference
+ * extracts it as, so e.g. 200 on an Int8 key is accepted): the pick stays only when |l - r| <= |tolerance|, else the row is
+ * null (default.rs:127-135).  |a - b| is abs_diff in the key's own type: exact unsigned for integers, a > b ? a - b :
+ * b - a in the float's precision (a NaN difference fails every comparison).  Key dtypes: Int/UInt 8-64 (8/16-bit searched as
+ * Int32, mod.rs:333-338) and Float32/64, one chunk per side; Bool keys: BL_ERR_UNSUPPORTED.
+ * by (n_by > 0): left_by[i] pairs with right_by[i], a numeric column (one chunk) or a string column (chunks) of the same type
+ * on both sides, flags 0; only right rows with equal `by` values are searched, in row order, exactly as bl_hash_join_keys
+ * with nulls_equal == 0 matches rows (floats -0 == +0, NaN == NaN; a null in any `by` column matches nothing).
+ * Errors: BL_ERR_DTYPE for `on` or `by` dtypes that differ (string vs numeric included); BL_ERR_INVALID for an unknown
+ * strategy, flags != 0, lengths that differ, a bad tolerance, n_by > 0 with a NULL array; BL_ERR_UNSUPPORTED for Bool `on`
+ * or `by` columns, an unsorted side, more than 2^32 - 2 rows on a side (both sides together with `by`). */
+bl_status bl_join_asof(const bl_column* left_on, const bl_column* right_on, const bl_sort_key* left_by, const bl_sort_key* right_by, int32_t n_by,
+                       int32_t strategy, int32_t allow_eq, const bl_column* tolerance, int32_t out_location, bl_column* out_right_idx);
+
 /* ---- K6: radix hash partition (multi-GPU exchange step) --------------------------------- */
 /* partition id = hash_to_partition(dirty_hash(key), n_partitions)
  *              = ((key * 0x55fbfd6bfc5458e9 mod 2^64) * n_partitions) >> 64   (hashing.rs:62-69,132-142),

@@ -757,6 +757,75 @@ def sort(by, cols: Sequence, descending=False, nulls_last=False, limit: int | No
     return _finish(list(outs)[:len(cs)], location)
 
 
+ASOF_STRATEGIES = {"backward": 0, "forward": 1, "nearest": 2}
+
+
+def _by_key(k, keep) -> BlSortKey:
+    """one `by` column -> a bl_sort_key with flags 0: a string column (StringColumn / DeviceStringColumn / list of chunks)
+    or a numeric one"""
+    if _is_string_key(k):
+        chunks = k if isinstance(k, list) else [k]
+        arr = _str_array(chunks)
+        keep.append(arr)
+        return BlSortKey(None, C.cast(arr, C.POINTER(BlStringColumn)), len(chunks), 0)
+    c = _as_col(k)
+    st = c.struct()
+    keep.append((c, st))
+    return BlSortKey(C.pointer(st), None, 0, 0)
+
+
+def join_asof(left_on, right_on, strategy: str = "backward", tolerance=None, allow_exact_matches: bool = True,
+              left_by=None, right_by=None, right_cols: Sequence = (), location: int = HOST):
+    """bl_join_asof: for each left row, the right row an asof search picks (see the header for the rule and the
+    precondition: sorted `on` columns, per group with `by`; otherwise B200Error with status UNSUPPORTED).
+    Returns the UInt32 index column as hash_join does: (values, valid) on the host, an OutColumn on the device.
+    left_by / right_by: a list of `by` columns per side (numeric columns, StringColumn or DeviceStringColumn).
+    tolerance: a scalar (converted exactly to the key dtype, or to Int32 for an 8/16-bit key as the reference does) or a
+    length-1 column of that dtype.
+    right_cols: payload columns of the right frame, gathered on the device at the index (bl_gather, or string_gather for
+    string columns); then the result is (index, [payloads])."""
+    if strategy not in ASOF_STRATEGIES:
+        raise ValueError(f"unknown asof strategy {strategy!r} (one of {', '.join(ASOF_STRATEGIES)})")
+    if (left_by is None) != (right_by is None):
+        raise ValueError("left_by and right_by must be given together")
+    left_by, right_by = list(left_by or []), list(right_by or [])
+    if len(left_by) != len(right_by):
+        raise ValueError(f"left_by has {len(left_by)} columns and right_by {len(right_by)}")
+    lc, rc = _as_col(left_on), _as_col(right_on)
+    tc = None
+    if tolerance is not None:
+        if isinstance(tolerance, (Column, OutColumn, tuple, np.ndarray)):
+            tc = _as_col(tolerance)
+        else:
+            if lc.dtype == BOOL:
+                raise ValueError("a tolerance needs a numeric key")
+            tdt = np.dtype(np.int32) if lc.dtype in (0, 1, 4, 5) else NP_OF[lc.dtype]      # Int8/16, UInt8/16: extracted as Int32
+            try:
+                t = np.array([tolerance], dtype=tdt)
+            except (OverflowError, ValueError, TypeError):
+                t = None
+            if t is None or not (t[0] == tolerance or (t[0] != t[0] and tolerance != tolerance)):
+                raise ValueError(f"tolerance {tolerance!r} is not representable as {tdt}")
+            tc = Column(t)
+    keep = []
+    n_by = len(left_by)
+    lb = (BlSortKey * max(n_by, 1))(*[_by_key(k, keep) for k in left_by])
+    rb = (BlSortKey * max(n_by, 1))(*[_by_key(k, keep) for k in right_by])
+    ls, rs = lc.struct(), rc.struct()
+    ts = tc.struct() if tc is not None else None
+    out = BlColumn()
+    out_loc = DEVICE if right_cols else location
+    _check(lib().bl_join_asof(C.byref(ls), C.byref(rs), lb if n_by else None, rb if n_by else None, C.c_int32(n_by),
+                              C.c_int32(ASOF_STRATEGIES[strategy]), C.c_int32(int(allow_exact_matches)), C.byref(ts) if ts is not None else None,
+                              C.c_int32(out_loc), C.byref(out)))
+    idx = _finish([out], out_loc)[0]
+    if not right_cols:
+        return idx
+    payloads = [string_gather(c, idx, location) if _is_string_key(c) else gather([c], idx, check_bounds=False, location=location)[0]
+                for c in right_cols]
+    return (idx.to_numpy() if location == HOST else idx), payloads
+
+
 def hash_partition(key, payload: Sequence, n_partitions: int, location: int = HOST):
     k = _as_col(key)
     ps = [_as_col(p) for p in payload]
