@@ -340,6 +340,38 @@ enum { BL_ASOF_BACKWARD = 0, BL_ASOF_FORWARD = 1, BL_ASOF_NEAREST = 2 };
 bl_status bl_join_asof(const bl_column* left_on, const bl_column* right_on, const bl_sort_key* left_by, const bl_sort_key* right_by, int32_t n_by,
                        int32_t strategy, int32_t allow_eq, const bl_column* tolerance, int32_t out_location, bl_column* out_right_idx);
 
+/* ---- inequality join  (IEJoin: _join_impl polars-ops/src/frame/join/mod.rs:243-270; iejoin/mod.rs:572-799) ---- */
+enum { BL_IE_LT = 0, BL_IE_LE = 1, BL_IE_GT = 2, BL_IE_GE = 3 };
+/* The reference's join_where with one or two inequality predicates (the planner's JoinType::IEJoin): left_on[k] ops[k]
+ * right_on[k] for k < n_pred (1 or 2).  The pair (i, j) is in the result iff left_on[k][i] ops[k] right_on[k][j] holds for
+ * every k, compared in the total order (NaN greatest and equal to NaN, -0.0 == +0.0: tot_lt / tot_le ...), and every
+ * predicate column is valid in both rows.  This is the set both serial algorithms compute (piecewise_merge_join_tuples
+ * mod.rs:667-799, iejoin_tuples :572-665) and the reference's own test rule, a cross join filtered by the predicates.
+ *   how = BL_JOIN_INNER  those pairs.
+ *   how = BL_JOIN_LEFT   those pairs plus one (i, null) for every left row without one, a row with a null predicate value
+ *                        included (append_unmatched_left, mod.rs:232-265).
+ * A right join is this call with the sides swapped, every operator flipped (< and >, <= and >=) and the outputs swapped
+ * (emit_unmatched_right_via_flip, mod.rs:279-296).  Semi, anti, full and any other `how`: BL_ERR_INVALID, as the reference
+ * rejects them for non-equi predicates.
+ * Outputs: two BL_UINT32 columns of one row per pair.  out_left_idx has no nulls; out_right_idx has a validity bitmap only
+ * for BL_JOIN_LEFT, with BL_IDX_NULL in its null slots.
+ * Order (the reference pins none; join_where documents that the row order is not preserved): pairs are grouped by left row,
+ * left rows ascending, an unmatched left row of a left join at its place.  The order inside one left row is deterministic
+ * (the same inputs give the same bytes) but unspecified.
+ * Quirk, not reproduced: the parallel path (iejoin_par_indices, mod.rs:331-458) skips a pair of blocks when their first /
+ * last x-values fail `<` / `<=` compared as AnyValue (mod.rs:372-400), a partial order for floats; with NaN x-values it can
+ * drop pairs that the serial algorithms and the cross-join rule keep.  This call follows the total-order rule.
+ * Columns: one chunk each; both sides of one predicate have the same dtype, the two predicates may differ.  Dtypes: Int/UInt
+ * 8-64, Float32/64.
+ * Device memory: with two predicates, a merge-sort tree of L x m x 8 bytes for m right rows valid in both predicate columns,
+ * L = 1 + ceil(log2 m) (about 2 GB at m = 1e7).  The pair count is known before the output is allocated.
+ * Errors: BL_ERR_DTYPE for dtypes that differ within a predicate (the reference's ComputeError, mod.rs:231-241);
+ * BL_ERR_UNSUPPORTED for a Bool column or more than 2^32 - 2 rows on a side; BL_ERR_INVALID for a NULL pointer, n_pred
+ * outside {1, 2}, an unknown operator or `how`, predicate columns of different lengths on one side; BL_ERR_OOM when the
+ * tree or the output (the message gives the pair count) does not fit in device memory. */
+bl_status bl_ie_join(const bl_column* left_on, const bl_column* right_on, const int32_t* ops, int32_t n_pred,
+                     int32_t how, int32_t out_location, bl_column* out_left_idx, bl_column* out_right_idx);
+
 /* ---- K6: radix hash partition (multi-GPU exchange step) --------------------------------- */
 /* partition id = hash_to_partition(dirty_hash(key), n_partitions)
  *              = ((key * 0x55fbfd6bfc5458e9 mod 2^64) * n_partitions) >> 64   (hashing.rs:62-69,132-142),

@@ -826,6 +826,51 @@ def join_asof(left_on, right_on, strategy: str = "backward", tolerance=None, all
     return (idx.to_numpy() if location == HOST else idx), payloads
 
 
+IE_OPS = {"<": 0, "<=": 1, ">": 2, ">=": 3}
+IE_FLIP = {"<": ">", "<=": ">=", ">": "<", ">=": "<="}
+
+
+def ie_join(left_on, right_on, ops, how: str = "inner", left_cols: Sequence = (), right_cols: Sequence = (), location: int = HOST):
+    """bl_ie_join: every (left row, right row) pair with left_on[k] ops[k] right_on[k] for each of one or two predicates,
+    compared in the total order, every predicate value non-null (see the header for the rule and the order).
+    left_on / right_on: a column or a list of one or two columns; ops: one of "<" "<=" ">" ">=" or a list of them.
+    how: "inner", "left" (plus (i, null) for every unmatched left row) or "right" (the left join with the sides swapped and
+    every operator flipped; then every unmatched right row appears once with a null left index).
+    Returns (left_idx, right_idx) as hash_join does.  With left_cols / right_cols, both sides are gathered on the device
+    (bl_gather, or string_gather for string columns) and the result is (left outputs, right outputs) as `join` returns."""
+    lon = list(left_on) if isinstance(left_on, list) else [left_on]
+    ron = list(right_on) if isinstance(right_on, list) else [right_on]
+    opl = list(ops) if isinstance(ops, (list, tuple)) else [ops]
+    if not 1 <= len(lon) <= 2 or len(ron) != len(lon) or len(opl) != len(lon):
+        raise ValueError(f"ie_join needs one or two predicates with one column per side and one operator each, got {len(lon)} left, "
+                         f"{len(ron)} right columns and {len(opl)} operators")
+    for op in opl:
+        if op not in IE_OPS:
+            raise ValueError(f"unknown inequality operator {op!r} (one of {', '.join(IE_OPS)})")
+    if how not in ("inner", "left", "right"):
+        raise ValueError(f"ie_join supports how = 'inner', 'left' or 'right', got {how!r}")
+    flip = how == "right"
+    if flip:
+        lon, ron, opl = ron, lon, [IE_FLIP[op] for op in opl]
+    lc, rc = [_as_col(c) for c in lon], [_as_col(c) for c in ron]
+    la, ra = _col_array(lc), _col_array(rc)
+    opa = (C.c_int32 * len(opl))(*[IE_OPS[op] for op in opl])
+    gather_after = bool(left_cols) or bool(right_cols)
+    out_loc = DEVICE if gather_after else location
+    ol, orr = BlColumn(), BlColumn()
+    _check(lib().bl_ie_join(la, ra, opa, C.c_int32(len(opl)), C.c_int32(JOINS["inner" if how == "inner" else "left"]), C.c_int32(out_loc),
+                            C.byref(ol), C.byref(orr)))
+    li, ri = _finish([ol, orr], out_loc)
+    if flip:
+        li, ri = ri, li
+    if not gather_after:
+        return li, ri
+
+    def take(cols, idx):
+        return [string_gather(c, idx, location) if _is_string_key(c) else gather([c], idx, check_bounds=False, location=location)[0] for c in cols]
+    return take(left_cols, li), take(right_cols, ri)
+
+
 def hash_partition(key, payload: Sequence, n_partitions: int, location: int = HOST):
     k = _as_col(key)
     ps = [_as_col(p) for p in payload]
