@@ -64,7 +64,7 @@ bl_status bl_gather(const bl_column* cols, int32_t n_cols, const bl_column* idx,
     std::vector<DevCol> in, o;
     for (int i = 0; i < n_cols; i++) in.push_back(import_column(&cols[i], 1));
     DevCol ix = import_column(idx, 1);
-    op_gather(in, ix, check_bounds != 0, o);
+    op_gather(in, ix, check_bounds != 0, o, true);      // a caller's index column may hold BL_IDX_NULL without a bitmap
     export_many(o, out_location, outs);
     BL_CATCH
 }

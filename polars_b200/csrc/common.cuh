@@ -151,7 +151,8 @@ DevCol op_elementwise(int op, const DevCol& lhs, const DevCol& rhs);
 DevCol op_compare(int op, const DevCol& lhs, const DevCol& rhs, bool missing);
 void op_filter(const std::vector<DevCol>& cols, const DevCol& mask, std::vector<DevCol>& outs);
 DevCol op_cmp_scalar_mask(const DevCol& col, int cmp_op, const DevCol& scalar);
-void op_gather(const std::vector<DevCol>& cols, const DevCol& idx, bool check_bounds, std::vector<DevCol>& outs);
+// find_sentinel: scan an index column without nulls for BL_IDX_NULL (implied by check_bounds)
+void op_gather(const std::vector<DevCol>& cols, const DevCol& idx, bool check_bounds, std::vector<DevCol>& outs, bool find_sentinel = false);
 bool dtype_is_small_int(int dt);
 DevCol op_cast_small_int(const DevCol& in, int to_dtype, bool bits);
 DevCol op_group_first_ids(const DevCol& key);

@@ -33,12 +33,11 @@ __global__ void __launch_bounds__(256) k_gather(GatherArgs args, const uint32_t*
 #pragma unroll
             for (int k = 0; k < 4; k++) if (r0 + k < m) { ix[k] = idx[r0 + k]; ok[k] = true; }
         }
-        if (NULLABLE) {
+        // the sentinel is never dereferenced, even on the path for index columns known to hold no nulls
 #pragma unroll
-            for (int k = 0; k < 4; k++) {
-                if (ok[k] && ix[k] == BL_IDX_NULL) ok[k] = false;
-                if (ok[k] && idx_valid != nullptr && !bit_get(idx_valid, r0 + k)) ok[k] = false;
-            }
+        for (int k = 0; k < 4; k++) {
+            if (ok[k] && ix[k] == BL_IDX_NULL) ok[k] = false;
+            if (NULLABLE && ok[k] && idx_valid != nullptr && !bit_get(idx_valid, r0 + k)) ok[k] = false;
         }
         for (int c = 0; c < args.ncols; c++) {
             const GatherCol col = args.c[c];
@@ -80,30 +79,38 @@ __global__ void __launch_bounds__(256) k_gather(GatherArgs args, const uint32_t*
     }
 }
 
-__global__ void k_check_bounds(const uint32_t* __restrict__ idx, const uint32_t* __restrict__ idx_valid, int64_t m, uint32_t len, int* bad) {
+// flags[0]: a non-null index >= len; flags[1]: a non-null slot holds the BL_IDX_NULL sentinel
+__global__ void k_check_idx(const uint32_t* __restrict__ idx, const uint32_t* __restrict__ idx_valid, int64_t m, uint32_t len, int* flags) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) {
-        uint32_t x = idx[i];
-        if (x == BL_IDX_NULL) continue;
         if (idx_valid != nullptr && !bit_get(idx_valid, i)) continue;
-        if (x >= len) *bad = 1;
+        uint32_t x = idx[i];
+        if (x == BL_IDX_NULL) flags[1] = 1;
+        else if (x >= len) flags[0] = 1;
     }
 }
 
-void op_gather(const std::vector<DevCol>& cols, const DevCol& idx, bool check_bounds, std::vector<DevCol>& outs) {
+void op_gather(const std::vector<DevCol>& cols, const DevCol& idx, bool check_bounds, std::vector<DevCol>& outs, bool find_sentinel) {
     PLB_REQUIRE(idx.dtype == BL_UINT32, BL_ERR_DTYPE, "gather: idx must be BL_UINT32 (IdxSize)");
     const int64_t m = idx.len;
     outs.clear();
     for (auto& c : cols)
         PLB_REQUIRE(dtype_size(c.dtype) == 8 || dtype_size(c.dtype) == 4, BL_ERR_UNSUPPORTED, std::string("gather: dtype ") + dtype_name(c.dtype) + " is outside the hot path");
-    if (check_bounds && m > 0) {
-        DevPtr bad = dev_alloc(4); dev_memset(bad->p, 0, 4);
-        for (auto& c : cols) {
-            PLB_LAUNCH("k4_check_bounds", k_check_bounds, grid_for(m, 256), 256, 0, (const uint32_t*)idx.v(), idx.vm(), m, (uint32_t)std::min<int64_t>(c.len, 0xFFFFFFFFll), as<int>(bad));
-        }
-        if (read_scalar(as<int>(bad))) fail(BL_ERR_BOUNDS, "gather: index out of bounds");
+    // nullable path when the idx column may carry nulls: a bitmap, a non-zero null count, or the BL_IDX_NULL sentinel.
+    // An index column without a bitmap that claims no nulls may still hold the sentinel: the bounds check finds it in
+    // the same pass, and callers that cannot rule it out ask for the scan (find_sentinel).
+    bool nullable = idx.validity != nullptr || idx.null_count != 0;
+    if (m > 0 && (check_bounds || (find_sentinel && !nullable))) {
+        int64_t len = 0xFFFFFFFFll;                  // no index is out of range for the sentinel scan alone
+        if (check_bounds)
+            for (auto& c : cols) len = std::min<int64_t>(len, c.len);
+        DevPtr flags = dev_alloc(8); dev_memset(flags->p, 0, 8);
+        PLB_LAUNCH("k4_check_idx", k_check_idx, grid_for(m, 256), 256, 0, (const uint32_t*)idx.v(), idx.vm(), m, (uint32_t)len, as<int>(flags));
+        int f[2];
+        PLB_CUDA(cudaMemcpyAsync(f, flags->p, 8, cudaMemcpyDeviceToHost, ctx().stream));
+        PLB_CUDA(cudaStreamSynchronize(ctx().stream));
+        if (f[0]) fail(BL_ERR_BOUNDS, "gather: index out of bounds");
+        nullable |= f[1] != 0;
     }
-    // nullable path when the idx column may carry nulls (bitmap or the BL_IDX_NULL sentinel)
-    const bool nullable = idx.validity != nullptr || idx.null_count != 0;
     for (auto& c : cols) {
         DevCol o = make_col(c.dtype, m, nullable || c.validity != nullptr);
         outs.push_back(o);
