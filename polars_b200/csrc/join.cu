@@ -683,12 +683,12 @@ static JoinBuilt join_build(const DevCol& build, bool nulls_equal, bool need_lis
         PLB_REQUIRE(cap <= (1ull << 32), BL_ERR_UNSUPPORTED, "join: build side too large for 32-bit slots");
         int shift = 64; for (uint64_t x = cap; x > 1; x >>= 1) shift--;
         B.tab = dev_alloc((size_t)(cap + 1) * 4);
-        PLB_LAUNCH("k7_join_init", k_fill_u32j, grid_for((int64_t)cap + 1, 256), 256, 0, as<uint32_t>(B.tab), J_NONE, (int64_t)cap + 1);
+        PLB_LAUNCH("k7_jc_init", k_fill_u32j, grid_for((int64_t)cap + 1, 256), 256, 0, as<uint32_t>(B.tab), J_NONE, (int64_t)cap + 1);
         const int fp_mode = nb < (1 << 24) - 1 ? 1 : 0;
         if (nb > 0) {
             const int grid = grid_for(nb, 256);
             const int ne = nulls_equal ? 1 : 0;
-#define JC_BUILD(E, CN) PLB_LAUNCH("k7_join_build", (k_jc_build<E, CN>), grid, 256, 0, as<uint32_t>(B.tab), (uint32_t)(cap - 1), shift, fp_mode, (uint32_t)cap, build.v(), build.vm(), nb, ne, as<uint32_t>(B.slot_of_row), as<int>(has_dups))
+#define JC_BUILD(E, CN) PLB_LAUNCH("k7_jc_build", (k_jc_build<E, CN>), grid, 256, 0, as<uint32_t>(B.tab), (uint32_t)(cap - 1), shift, fp_mode, (uint32_t)cap, build.v(), build.vm(), nb, ne, as<uint32_t>(B.slot_of_row), as<int>(has_dups))
             if (dt == BL_FLOAT64) JC_BUILD(8, 1); else if (dt == BL_FLOAT32) JC_BUILD(4, 2); else if (elem == 8) JC_BUILD(8, 0); else JC_BUILD(4, 0);
 #undef JC_BUILD
         }

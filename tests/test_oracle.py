@@ -1,9 +1,12 @@
 """CPU tests (-m "not gpu"): pin the oracle against the reference's golden vectors and
 cross-check it against independent engines (pyarrow Acero, numpy) on random inputs."""
+import zlib
+
 import numpy as np
 import pyarrow as pa
 import pytest
 
+import join_keys
 import oracle
 from helpers import IDX_NULL, OracleImpl, assert_close, col, pairs_sorted, run_group_by_kat, run_join_kat, sort_groups
 
@@ -370,6 +373,85 @@ def test_full_join_vs_bruteforce(nl, nr, krange, nulls_equal):
     probe_side = ri if not (nl > nr) else li
     k = int((probe_side != NUL).sum())
     assert (probe_side[:k] != NUL).all() and np.all(np.diff(probe_side[:k].astype(np.int64)) >= 0) and (probe_side[k:] == NUL).all()
+
+
+def bruteforce_join(lk, lv, rk, rv, how, nulls_equal, order="none"):
+    """The reference's tuple sequence from its rules alone (hash_join/mod.rs:41-50, single_keys_outer.rs:100-260,
+    single_keys_semi_anti.rs:8-140, join/mod.rs:577-642, dispatch_left_right.rs:142-170), over join_keys.canon keys.
+    Returns (left idx, right idx) as lists; IDX_NULL marks a missing side."""
+    NUL = int(IDX_NULL)
+    lc, rc = join_keys.canon(lk, lv), join_keys.canon(rk, rv)
+
+    def rows_by_key(c):
+        d = {}
+        for j, x in enumerate(c):
+            if x is not None or nulls_equal:
+                d.setdefault(x, []).append(j)
+        return d
+
+    def left_join(pc, bc):           # every probe row in order; its matches ascending, or one miss
+        d = rows_by_key(bc)
+        out = []
+        for i, x in enumerate(pc):
+            m = d.get(x, []) if (x is not None or nulls_equal) else []
+            out += [(i, j) for j in m] or [(i, NUL)]
+        return out
+
+    if how in ("semi", "anti"):
+        d = rows_by_key(rc)
+        hit = [(x is not None or nulls_equal) and x in d for x in lc]
+        return [i for i, h in enumerate(hit) if h == (how == "semi")], []
+    swapped = not (len(lc) > len(rc)) if how in ("inner", "full") else False
+    pc, bc = (rc, lc) if swapped else (lc, rc)
+    seq = left_join(pc, bc)
+    if how == "inner":
+        seq = [t for t in seq if t[1] != NUL]
+    if how == "full":
+        hit = {j for _, j in seq}
+        seq += [(NUL, j) for j in range(len(bc)) if j not in hit]
+    if swapped:
+        seq = [(b, p) for p, b in seq]
+    if order in ("left", "left_right") and how == "inner":
+        seq = sorted(seq, key=lambda t: t[0])
+    elif order in ("right", "right_left") and how in ("inner", "left"):
+        seq = sorted(seq, key=lambda t: t[1])
+    return [t[0] for t in seq], [t[1] for t in seq]
+
+
+def _full_range_cases():
+    cases = []
+    for dt in join_keys.DTYPES:
+        for dups in ("unique", "k", "hot", "dense"):
+            if dups == "dense" and dt not in join_keys.INT_DTYPES:
+                continue
+            for nulls in (0, 0.04):
+                cases.append((dt, dups, nulls))
+    return cases
+
+
+@pytest.mark.parametrize("dtype,dups,nulls", _full_range_cases())
+def test_join_full_range_vs_bruteforce(dtype, dups, nulls):
+    """The oracle's join (every how, both nulls_equal, every maintain_order) against the brute-force restatement above,
+    on the key columns of tests/join_keys.py: the dtype's whole range with MIN / MAX / 0 / -1, UInt64 2^63 and 2^64 - 1,
+    NaN payloads of both signs, +-0.0, +-inf and subnormals.  These are the inputs the GPU join is compared with the
+    oracle on."""
+    rng = np.random.default_rng(zlib.crc32(f"{dtype}/{dups}/{nulls}".encode()))
+    small = np.dtype(dtype).itemsize == 1
+    nr = 200 if small else 700
+    if dups == "dense":
+        rk, rv = join_keys.keys(rng, dtype, nr, "unique", nulls=nulls, dense=min(3 * nr, 256) if small else 3 * nr)
+    else:
+        rk, rv = join_keys.keys(rng, dtype, nr, dups, k={"unique": 1, "k": 3, "hot": 40}[dups], nulls=nulls)
+    valid_rk = rk if rv is None else rk[rv]
+    for nl in (2 * nr + 1, nr // 2, nr):            # left probes / right probes / a tie (right probes)
+        lk, lv = join_keys.probe(rng, valid_rk, nl, nulls=nulls, dense_edges=dups == "dense")
+        for nulls_equal in (False, True):
+            for how, orders in (("inner", ("none", "left", "left_right", "right", "right_left")),
+                                ("left", ("none", "left", "right", "right_left")), ("full", ("none",)), ("semi", ("none",)), ("anti", ("none",))):
+                for order in orders:
+                    eli, eri = bruteforce_join(lk, lv, rk, rv, how, nulls_equal, order)
+                    li, ri = oracle.hash_join(lk, rk, lv, rv, how, nulls_equal, order, 3)
+                    assert li.tolist() == eli and ri.tolist() == eri, (nl, how, nulls_equal, order)
 
 
 def test_first_last_var_std_vs_numpy():
