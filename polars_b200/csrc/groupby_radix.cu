@@ -8,8 +8,11 @@
 //   pass 1  k_gbr_scatter   every CTA sorts a 2048-row tile by bucket in shared memory as ROW-MAJOR records
 //                           [key, v0, v1, ...] and writes each (tile, bucket) run with ONE cp.async.bulk (TMA)
 //                           shared->global copy (runs padded to an even record count with a GB_EMPTY-key record so both
-//                           ends stay 16-byte aligned).  Past 512 buckets the runs shrink to single records and the
-//                           tile is written with coalesced 8-byte stores instead (no padding).
+//                           ends stay 16-byte aligned).  Past 512 buckets the runs shrink to single records:
+//           k_gbr_scatter_wc    instead collects every bucket's rows in a 4-record chunk buffer in shared memory
+//                           (software write-combining) and writes each full chunk with one cp.async.bulk copy of
+//                           whole 32-byte sectors; when a buffer per bucket does not fit one CTA's shared memory,
+//                           k_gbr_scatter writes the sorted tile with coalesced 8-byte stores (no padding).
 //   pass 2  k_gbr_agg       one CTA per bucket: the bucket's record stream is staged into shared memory by
 //                           cp.async.bulk (TMA) global->shared copies on an mbarrier ring (a producer warp issues,
 //                           31 consumer warps each release their slice of a stage on an `empty` mbarrier as soon as it
@@ -37,7 +40,7 @@ constexpr int GBR_NCW = 31, GBR_NCT = GBR_NCW * 32;                             
 
 struct GbRadixDev {
     uint64_t* recs;                 // record streams, bucket b at recs + off[b] * roww
-    const unsigned long long* off;  // first record of bucket b (even)
+    const unsigned long long* off;  // first record of bucket b (even; a multiple of GBR_WC_F for the write-combining scatter)
     unsigned* cursor;               // records written to bucket b so far (pads included)
     unsigned* counts;               // pass 0: rows of bucket b
     int logB, roww;
@@ -77,8 +80,10 @@ __global__ void __launch_bounds__(512) k_gbr_hist(const void* __restrict__ keys,
     __syncthreads();
     for (int i = threadIdx.x; i < B; i += blockDim.x) if (h_s[i]) atomicAdd(&counts[i], h_s[i]);
 }
-// bucket capacities (worst-case padding: one pad record per tile that touches the bucket) -> exclusive offsets, one CTA
-__global__ void __launch_bounds__(1024) k_gbr_offsets(const unsigned* __restrict__ counts, int B, unsigned long long ntiles, int pad, unsigned long long* __restrict__ off, unsigned* __restrict__ cursor) {
+// bucket capacities -> exclusive offsets, one CTA.  Worst-case padding: `pad_each` records for each of up to `pad_units`
+// writers that touch the bucket (tile runs: one per tile; write-combining: F - 1 per CTA), rounded up to `align` records.
+__global__ void __launch_bounds__(1024) k_gbr_offsets(const unsigned* __restrict__ counts, int B, unsigned long long pad_units, unsigned pad_each, unsigned align,
+                                                      unsigned long long* __restrict__ off, unsigned* __restrict__ cursor) {
     __shared__ unsigned long long wsum[32];
     __shared__ unsigned long long carry_s;
     if (threadIdx.x == 0) carry_s = 0;
@@ -87,7 +92,7 @@ __global__ void __launch_bounds__(1024) k_gbr_offsets(const unsigned* __restrict
     for (int base = 0; base < B; base += 1024) {
         const int i = base + threadIdx.x;
         unsigned long long c = 0;
-        if (i < B) { c = counts[i]; if (pad) c += c < ntiles ? c : ntiles; c = (c + 1ull) & ~1ull; cursor[i] = 0; }      // even: every stream starts 16-byte aligned
+        if (i < B) { c = counts[i]; c += (c < pad_units ? c : pad_units) * pad_each; c = (c + align - 1) & ~(unsigned long long)(align - 1); cursor[i] = 0; }   // every stream starts 16-byte (even) / 32-byte (F) aligned
         unsigned long long x = c;
         for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= (unsigned)o) x += y; }
         if (lane == 31) wsum[warp] = x;
@@ -236,6 +241,120 @@ __global__ void __launch_bounds__(GBR_THREADS) k_gbr_scatter(const __grid_consta
     if (BULK) bulk_wait0();
 }
 
+// ---------------------------------------------------------------------------- pass 1, many buckets: write-combining buffers
+// A persistent CTA keeps one chunk buffer of F records per bucket in shared memory.  Rows take a slot s in their bucket's
+// chunk sequence with one shared-memory atomic; in round r the rows of chunk s / F == r land in the buffer, and every chunk
+// that round completed leaves with one global reservation (atomicAdd(cursor, F)) and one cp.async.bulk shared->global
+// copy.  Bucket streams start on whole chunks (k_gbr_offsets aligns them to F records), so every store is whole 32-byte
+// sectors.  The next tile's keys and values load into registers while the current tile is bucketed.  At the end each
+// CTA flushes its partial chunks padded with GB_EMPTY-key records (pass 2 skips them).
+constexpr int GBR_WC_THREADS = 256, GBR_WC_F = 4;
+template <int ROWW> constexpr int gbr_wc_rpt() { return ROWW <= 3 ? 8 : 4; }
+template <int ROWW, int KEY_ELEM, int RPT>
+__device__ __forceinline__ void gbr_wc_load(const GbBatch& Bt, int64_t base, uint64_t (&k)[RPT], uint64_t (&v)[ROWW > 1 ? ROWW - 1 : 1][RPT]) {
+#pragma unroll
+    for (int j = 0; j < RPT / 2; j++) {
+        const int64_t r0 = base + 2 * (int64_t)(j * GBR_WC_THREADS + threadIdx.x);
+        gbr_load_pair<KEY_ELEM>(Bt.keys, r0, Bt.n, k[2 * j], k[2 * j + 1]);
+#pragma unroll
+        for (int c = 0; c < ROWW - 1; c++) gbr_load_pair_rt(Bt.cols[c].values, Bt.cols[c].elem, r0, Bt.n, v[c][2 * j], v[c][2 * j + 1]);
+    }
+}
+
+template <int ROWW, int KEY_ELEM, int KEY_CANON>
+__global__ void __launch_bounds__(GBR_WC_THREADS, 2) k_gbr_scatter_wc(const __grid_constant__ GbLayout L, const __grid_constant__ GbBatch Bt, const __grid_constant__ GbRadixDev R) {
+    constexpr int THREADS = GBR_WC_THREADS, F = GBR_WC_F, RPT = gbr_wc_rpt<ROWW>(), T = THREADS * RPT, NC = ROWW - 1, NCX = NC > 0 ? NC : 1, CH = F * ROWW;
+    constexpr unsigned NONE = 0xFFFFFFFFu;
+    const int logB = R.logB, B = 1 << logB, tid = threadIdx.x;
+    extern __shared__ __align__(16) uint64_t gbr_smem[];
+    uint64_t* buf = gbr_smem;                                                       // B chunks of CH words
+    unsigned* fill = reinterpret_cast<unsigned*>(buf + (size_t)B * CH);             // records in the bucket's open chunk (< F between tiles)
+    const int64_t n = Bt.n, ntiles = (n + T - 1) / T;
+    for (int p = tid; p < B; p += THREADS) fill[p] = 0;
+    uint64_t k[RPT], v[NCX][RPT], kn[RPT], vn[NCX][RPT];
+    if ((int64_t)blockIdx.x < ntiles) gbr_wc_load<ROWW, KEY_ELEM, RPT>(Bt, (int64_t)blockIdx.x * T, kn, vn);
+    for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+#pragma unroll
+        for (int e = 0; e < RPT; e++) { k[e] = kn[e];
+#pragma unroll
+                                        for (int c = 0; c < NC; c++) v[c][e] = vn[c][e]; }
+        if (tile + gridDim.x < ntiles) gbr_wc_load<ROWW, KEY_ELEM, RPT>(Bt, (tile + gridDim.x) * T, kn, vn);
+        const int64_t base = tile * T;
+        unsigned pk[RPT];        // bucket << 16 | slot in the bucket's chunk sequence of this tile;  NONE = no row
+#pragma unroll
+        for (int e = 0; e < RPT; e++) {
+            const int64_t r = base + 2 * (int64_t)((e >> 1) * THREADS + tid) + (e & 1);
+            pk[e] = NONE;
+            if (r < n) {
+                k[e] = canon_key<KEY_CANON>(k[e]);
+                if (k[e] == GB_EMPTY) {      // the GB_EMPTY key is the pad marker of the record streams: its (rare) rows aggregate right here
+                    uint64_t raw[NCX];
+#pragma unroll
+                    for (int c = 0; c < NC; c++) raw[c] = v[c][e];
+                    gbr_apply_special(L, Bt, R.special, raw);
+                } else pk[e] = (unsigned)(table_hash(k[e]) >> (64 - logB)) << 16;
+            }
+        }
+        __syncthreads();                 // the previous tile's owners have reset fill[]
+        unsigned last = 0;               // highest chunk index among this thread's rows
+#pragma unroll
+        for (int e = 0; e < RPT; e++)
+            if (pk[e] != NONE) { const unsigned s = atomicAdd(&fill[pk[e] >> 16], 1u); pk[e] |= s; last = max(last, s / F); }
+        bulk_wait_read0();               // this thread's copies of the previous tile have finished reading their buffers
+        __syncthreads();
+        for (unsigned r = 0;; r++) {
+#pragma unroll
+            for (int e = 0; e < RPT; e++) {
+                const unsigned s = pk[e] & 0xFFFFu;
+                if (pk[e] == NONE || s / F != r) continue;
+                uint64_t* rec = buf + (size_t)(pk[e] >> 16) * CH + (s % F) * ROWW;
+                rec[0] = k[e];
+#pragma unroll
+                for (int c = 0; c < NC; c++) rec[1 + c] = v[c][e];
+            }
+            fence_async_smem();
+            const bool more = __syncthreads_or(last > r);
+            // owners (bucket p belongs to thread p % THREADS) write out the chunks this round completed
+            const unsigned full = (r + 1) * F;
+            for (int p0 = 0; p0 < B; p0 += 4 * THREADS) {
+                unsigned g[4];
+#pragma unroll
+                for (int q = 0; q < 4; q++) {            // reservations first, so their latencies overlap
+                    const int p = p0 + q * THREADS + tid;
+                    g[q] = NONE;
+                    if (p < B) {
+                        const unsigned f = fill[p];
+                        if (f >= full) g[q] = atomicAdd(&R.cursor[p], (unsigned)F);
+                        if (!more) fill[p] = f % F;
+                    }
+                }
+#pragma unroll
+                for (int q = 0; q < 4; q++) {
+                    const int p = p0 + q * THREADS + tid;
+                    if (g[q] != NONE) bulk_s2g(R.recs + (R.off[p] + g[q]) * ROWW, buf + (size_t)p * CH, CH * 8);
+                }
+            }
+            bulk_commit();
+            if (!more) break;
+            bulk_wait_read0();
+            __syncthreads();
+        }
+    }
+    // partial chunks, padded to F records with GB_EMPTY keys (their buffers are not in flight: a chunk that left in the
+    // last round was full, which leaves its bucket's buffer empty)
+    __syncthreads();
+    for (int p = tid; p < B; p += THREADS) {
+        const unsigned f = fill[p];
+        if (f == 0) continue;
+        for (unsigned i = f; i < F; i++) buf[(size_t)p * CH + i * ROWW] = GB_EMPTY;
+        fence_async_smem();
+        const unsigned g = atomicAdd(&R.cursor[p], (unsigned)F);
+        bulk_s2g(R.recs + (R.off[p] + g) * ROWW, buf + (size_t)p * CH, CH * 8);
+    }
+    bulk_commit();
+    bulk_wait0();
+}
+
 // ---------------------------------------------------------------------------- pass 2: TMA ring -> shared-memory table -> dense output
 struct GbDenseDev { uint64_t* keys; uint32_t* first; uint32_t* len; uint64_t* words; int64_t Gb; unsigned long long* cursor; };
 
@@ -359,6 +478,21 @@ __global__ void k_gbr_append_special(const uint64_t* __restrict__ special, int n
 // =============================================================================================
 constexpr int GBR_RPT_BULK = 4, GBR_RPT_PLAIN = 4;      // 8 rows per thread (4096-row tiles, 1 CTA / SM) was slower
 static int64_t gbr_tile_rows(bool bulk) { return (int64_t)GBR_THREADS * (bulk ? GBR_RPT_BULK : GBR_RPT_PLAIN); }
+static size_t gbr_wc_smem(int B, int roww) { return (size_t)B * (GBR_WC_F * roww * 8 + 4); }
+// write-combining scatter: grid = the CTAs that fit at once (persistent; k_gbr_offsets pads for each of them)
+template <int ROWW, int KEY_ELEM, int KEY_CANON>
+static void scatter_wc_grid(int B, int& grid) {
+    auto kfn = k_gbr_scatter_wc<ROWW, KEY_ELEM, KEY_CANON>;
+    const size_t smem = gbr_wc_smem(B, ROWW);
+    PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int occ = 0;
+    PLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kfn, GBR_WC_THREADS, smem));
+    grid = ctx().sm_count * std::max(occ, 1);
+}
+template <int ROWW, int KEY_ELEM, int KEY_CANON>
+static void launch_scatter_wc(const GbLayout& L, const GbBatch& Bt, const GbRadixDev& R, int grid) {
+    PLB_LAUNCH("k5r_scatter", (k_gbr_scatter_wc<ROWW, KEY_ELEM, KEY_CANON>), grid, GBR_WC_THREADS, gbr_wc_smem(1 << R.logB, ROWW), L, Bt, R);
+}
 template <int ROWW, int KEY_ELEM, int KEY_CANON>
 static void launch_scatter(const GbLayout& L, const GbBatch& Bt, const GbRadixDev& R, bool bulk) {
     const int B = 1 << R.logB;
@@ -449,10 +583,23 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
     }
     const int B = 1 << logB;
     const bool bulk = logB <= 9;
+    // many buckets: write-combining buffers when a chunk buffer per bucket fits one CTA's shared memory, else the
+    // tile is written with coalesced stores
+    int smem_optin = 0;
+    PLB_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx().device));
+    const bool wc = !bulk && gbr_wc_smem(B, roww) <= (size_t)smem_optin;
     const int64_t ntiles = (n + gbr_tile_rows(bulk) - 1) / gbr_tile_rows(bulk);
-    const int64_t rec_rows = n + (bulk ? std::min<int64_t>(n, (int64_t)B * ntiles) : 0) + 2 * B + 16;
     const int elem = dtype_size(key.dtype);
     const int canon = key.dtype == BL_FLOAT64 ? 1 : (key.dtype == BL_FLOAT32 ? 2 : 0);
+#define GBR_KEYS(CALL) do { if (elem == 8) { if (canon == 1) { CALL(8, 1); } else { CALL(8, 0); } } else { if (canon == 2) { CALL(4, 2); } else { CALL(4, 0); } } } while (0)
+#define GBR_ROWW(FN, E, CN, ...) do { switch (roww) { case 1: FN<1, E, CN>(__VA_ARGS__); break; case 2: FN<2, E, CN>(__VA_ARGS__); break; case 3: FN<3, E, CN>(__VA_ARGS__); break; \
+                                                      case 4: FN<4, E, CN>(__VA_ARGS__); break; default: FN<5, E, CN>(__VA_ARGS__); break; } } while (0)
+    int wc_grid = 0;
+#define WCGRID(E, CN) GBR_ROWW(scatter_wc_grid, E, CN, B, wc_grid)
+    if (wc) GBR_KEYS(WCGRID);
+#undef WCGRID
+    const int64_t pad_rows = bulk ? std::min<int64_t>(n, (int64_t)B * ntiles) : wc ? std::min<int64_t>(n, (int64_t)B * wc_grid) * (GBR_WC_F - 1) : 0;
+    const int64_t rec_rows = n + pad_rows + (wc ? GBR_WC_F : 2) * (int64_t)B + 16;
     DevPtr recs, ctl;
     try {
         recs = dev_alloc((size_t)rec_rows * roww * 8);
@@ -473,15 +620,15 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
     }
     dev_memset(status->p, 0, 4);
     const int hgrid = ctx().sm_count * 4;
-#define GBR_KEYS(CALL) do { if (elem == 8) { if (canon == 1) { CALL(8, 1); } else { CALL(8, 0); } } else { if (canon == 2) { CALL(4, 2); } else { CALL(4, 0); } } } while (0)
 #define HIST(E, CN) PLB_LAUNCH("k5r_histogram", (k_gbr_hist<E, CN>), hgrid, 512, (size_t)B * 4, key.v(), n, logB, R.counts)
     GBR_KEYS(HIST);
 #undef HIST
-    PLB_LAUNCH("k5r_offsets", k_gbr_offsets, 1, 1024, 0, R.counts, B, (unsigned long long)ntiles, bulk ? 1 : 0, const_cast<unsigned long long*>(R.off), R.cursor);
-#define SCAT(E, CN) do { switch (roww) { case 1: launch_scatter<1, E, CN>(Lb, Bt, R, bulk); break; case 2: launch_scatter<2, E, CN>(Lb, Bt, R, bulk); break; case 3: launch_scatter<3, E, CN>(Lb, Bt, R, bulk); break; \
-                                          case 4: launch_scatter<4, E, CN>(Lb, Bt, R, bulk); break; default: launch_scatter<5, E, CN>(Lb, Bt, R, bulk); break; } } while (0)
+    if (wc) PLB_LAUNCH("k5r_offsets", k_gbr_offsets, 1, 1024, 0, R.counts, B, (unsigned long long)wc_grid, (unsigned)(GBR_WC_F - 1), (unsigned)GBR_WC_F, const_cast<unsigned long long*>(R.off), R.cursor);
+    else PLB_LAUNCH("k5r_offsets", k_gbr_offsets, 1, 1024, 0, R.counts, B, (unsigned long long)ntiles, bulk ? 1u : 0u, 2u, const_cast<unsigned long long*>(R.off), R.cursor);
+#define SCAT(E, CN) do { if (wc) GBR_ROWW(launch_scatter_wc, E, CN, Lb, Bt, R, wc_grid); else GBR_ROWW(launch_scatter, E, CN, Lb, Bt, R, bulk); } while (0)
     GBR_KEYS(SCAT);
 #undef SCAT
+#undef GBR_ROWW
 #undef GBR_KEYS
     // dense output, sized by a generous bound on the group count (overflow -> status -> fall back)
     const int64_t Gb = std::max<int64_t>(1024, std::min<int64_t>(n + 1, 3 * est_groups + (1 << 16)));
@@ -496,7 +643,8 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
     }
     PLB_LAUNCH("k5r_special", k_gbr_append_special, 1, 32, 0, R.special, L.n_words, D, as<int>(status));
     const int st = read_scalar(as<int>(status));      // also orders ctl_init / recs lifetimes
-    if (getenv("BL_K5_DEBUG")) fprintf(stderr, "[k5r] rows=%lld est_groups=%lld buckets=%d slots=%u bulk=%d status=%d\n", (long long)n, (long long)est_groups, B, S, (int)bulk, st);
+    if (getenv("BL_K5_DEBUG")) fprintf(stderr, "[k5r] rows=%lld est_groups=%lld buckets=%d slots=%u bulk=%d store=%s status=%d\n", (long long)n, (long long)est_groups, B, S, (int)bulk,
+                                      bulk ? "runs" : wc ? "wc" : "coalesced", st);
     if (st != 0) { dense = GbDense{}; dev_memset(status->p, 0, 4); return false; }
     dense.ready = true;
     rows_seen = n;
