@@ -50,18 +50,6 @@ __device__ __forceinline__ uint64_t tbl_load(const uint64_t* p, uint64_t pol, in
     else v = __ldcg(reinterpret_cast<const unsigned long long*>(p));
     return v;
 }
-__device__ __forceinline__ void red_add_u64(uint64_t* p, uint64_t v, uint64_t pol, bool hint) {
-    if (hint) asm volatile("red.global.add.L2::cache_hint.u64 [%0], %1, %2;" :: "l"(p), "l"(v), "l"(pol) : "memory");
-    else atomicAdd(reinterpret_cast<unsigned long long*>(p), (unsigned long long)v);
-}
-__device__ __forceinline__ void red_add_f64(uint64_t* p, double v, uint64_t pol, bool hint) {
-    if (hint) asm volatile("red.global.add.L2::cache_hint.f64 [%0], %1, %2;" :: "l"(p), "d"(v), "l"(pol) : "memory");
-    else atomicAdd(reinterpret_cast<double*>(p), v);
-}
-__device__ __forceinline__ void red_add_u32(uint32_t* p, uint32_t v, uint64_t pol, bool hint) {
-    if (hint) asm volatile("red.global.add.L2::cache_hint.u32 [%0], %1, %2;" :: "l"(p), "r"(v), "l"(pol) : "memory");
-    else atomicAdd(p, v);
-}
 
 // claim / find the entry of `key`, continuing from slot `slot` whose key word `k` has already been
 // loaded (the first probes of all rows of an iteration are issued together).
@@ -96,6 +84,26 @@ __device__ __forceinline__ uint64_t* gb_special(const GbTableDev& T, int which) 
 __device__ __forceinline__ uint64_t* gb_wp(const GbTableDev& T, uint64_t* e, int w) {
     return e + gb_woff(T.pw ? (int64_t)(e - T.entries) : 0, w, T.ws, T.pw);
 }
+// one row into the global-table entry `e`: len, first, then every accumulator word (val, skip_pair: see gb_apply_words)
+template <int MAXC, class Val>
+__device__ __forceinline__ void gb_apply_row(const GbLayout& L, const GbTableDev& T, const GbBatch& B, uint64_t* e, int64_t row, Val val, uint64_t pol = 0, bool hint = false, bool skip_pair = false) {
+    if (L.need_len && !skip_pair) red_add_u32(reinterpret_cast<uint32_t*>(gb_wp(T, e, 1)), 1u, pol, hint);
+    if (L.need_first) atomicMin(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)) + 1, B.row_base + (uint32_t)row);
+    gb_apply_words<MAXC>(L, B, row, val, [&](int w) { return gb_wp(T, e, 2 + w); }, pol, hint, skip_pair);
+}
+// the odd last row of a batch (the row loops take row pairs): thread 0 of CTA 0 applies it to the global table
+__device__ __forceinline__ void gb_tail_row(const GbLayout& L, const GbTableDev& T, const GbBatch& B) {
+    if (!(B.n & 1) || blockIdx.x != 0 || threadIdx.x != 0) return;
+    const int64_t row = B.n - 1;
+    const bool kvalid = B.key_validity == nullptr || bit_get(B.key_validity, row);
+    const uint64_t key = load_key_rt(B.keys, B.key_dtype, row);
+    const bool regular = kvalid && key != GB_EMPTY;
+    const bool mine = !T.pass_bits || (regular ? (int)(table_hash(key) >> (64 - T.pass_bits)) == T.pass_id : T.pass_id == 0);
+    uint64_t* e = !mine ? nullptr : (!kvalid ? gb_special(T, 0) : (key == GB_EMPTY ? gb_special(T, 1) : gb_find_or_insert(T, key)));
+    if (e) gb_apply_row<0>(L, T, B, e, row, [&](int c) {
+        return B.cols[c].elem == 8 ? reinterpret_cast<const uint64_t*>(B.cols[c].values)[row] : (uint64_t)reinterpret_cast<const uint32_t*>(B.cols[c].values)[row];
+    });
+}
 // ---- bulk reduce (TMA): one cp.reduce.async.bulk adds the 16-byte shared-memory cell {1, v} to the table cell {len | first, sum}.
 //      Key load + this + 1 RED.F64 replaces key load + 3 REDs per row: the L2 / LSU RED rate is the ceiling of the table
 //      update and the TMA unit is a second, otherwise idle, path into the same L2 atomic units (sm_90 and later).  SASS: UBLKRED.G.S.ADD.U64 (uniform datapath: ptxas serialises the lanes).
@@ -103,20 +111,6 @@ __device__ __forceinline__ void bulk_add_u64x2(uint64_t* dst, const uint64_t* sr
     const uint32_t sa = (uint32_t)__cvta_generic_to_shared(src_smem);
     if (hint) asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.L2::cache_hint.add.u64 [%0], [%1], 16, %2;" :: "l"(dst), "r"(sa), "l"(pol) : "memory");
     else asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], 16;" :: "l"(dst), "r"(sa) : "memory");
-}
-
-__device__ __forceinline__ void gb_apply(int op, uint64_t* addr, int dtype, uint64_t raw, bool valid, uint64_t pol = 0, bool hint = false) {
-    switch (op) {
-        case W_ADD_INT: { uint64_t v = raw_to_int(dtype, raw); if (valid && v) red_add_u64(addr, v, pol, hint); break; }
-        case W_ADD_F64: { double f = raw_to_f64(dtype, raw); if (valid && f != 0.0) red_add_f64(addr, f, pol, hint); break; }
-        case W_MIN_S64: if (valid) atomicMin(reinterpret_cast<long long*>(addr), (long long)raw_to_int(dtype, raw)); break;
-        case W_MAX_S64: if (valid) atomicMax(reinterpret_cast<long long*>(addr), (long long)raw_to_int(dtype, raw)); break;
-        case W_MIN_U64: if (valid) atomicMin(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)raw); break;
-        case W_MAX_U64: if (valid) atomicMax(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)raw); break;
-        case W_MIN_F64: { double f = raw_to_f64(dtype, raw); if (valid && f == f) atomicMin(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)f64_to_ordered(f)); break; }
-        case W_MAX_F64: { double f = raw_to_f64(dtype, raw); if (valid && f == f) atomicMax(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)f64_to_ordered(f)); break; }
-        default: if (!valid) atomicAdd(reinterpret_cast<unsigned long long*>(addr), 1ull); break;   // W_NULLCNT
-    }
 }
 
 // ---------------------------------------------------------------------------- K5 main kernel
@@ -146,15 +140,10 @@ __global__ void __launch_bounds__(256) k_gb_consume(const __grid_constant__ GbLa
         for (int u = 0; u < PAIRS; u++) {
             const int64_t p = p0 + u * gstride;
             if (p < npairs) {
-                if (KEY_ELEM == 8) { ulonglong2 t = ld_stream_u64x2(reinterpret_cast<const uint64_t*>(B.keys) + 2 * p); kraw[2 * u] = t.x; kraw[2 * u + 1] = t.y; }
-                else { uint2 t = ld_stream_u32x2(reinterpret_cast<const uint32_t*>(B.keys) + 2 * p); kraw[2 * u] = t.x; kraw[2 * u + 1] = t.y; }
+                gb_load_pair<KEY_ELEM>(B.keys, 2 * p, kraw[2 * u], kraw[2 * u + 1]);
 #pragma unroll
-                for (int c = 0; c < MAXC; c++) {
-                    if (c < L.n_cols) {
-                        if (B.cols[c].elem == 8) { ulonglong2 t = ld_stream_u64x2(reinterpret_cast<const uint64_t*>(B.cols[c].values) + 2 * p); raw[c][2 * u] = t.x; raw[c][2 * u + 1] = t.y; }
-                        else { uint2 t = ld_stream_u32x2(reinterpret_cast<const uint32_t*>(B.cols[c].values) + 2 * p); raw[c][2 * u] = t.x; raw[c][2 * u + 1] = t.y; }
-                    }
-                }
+                for (int c = 0; c < MAXC; c++)
+                    if (c < L.n_cols) gb_load_pair_rt(B.cols[c].values, B.cols[c].elem, 2 * p, raw[c][2 * u], raw[c][2 * u + 1]);
             }
         }
         // first probe of every row
@@ -206,42 +195,13 @@ __global__ void __launch_bounds__(256) k_gb_consume(const __grid_constant__ GbLa
             uint64_t* e = ent[r];
             if (e == nullptr) continue;
             const int64_t row = 2 * (p0 + (r >> 1) * gstride) + (r & 1);
-            uint64_t* const w1 = gb_wp(T, e, 1);
-            if (L.need_len && !bulk_lane) red_add_u32(reinterpret_cast<uint32_t*>(w1), 1u, pol, hint);
-            if (L.need_first) atomicMin(reinterpret_cast<unsigned*>(w1) + 1, B.row_base + (uint32_t)row);
-#pragma unroll
-            for (int c = 0; c < MAXC; c++) {
-                if (c < L.n_cols) {
-                    const bool valid = B.cols[c].validity == nullptr || bit_get(B.cols[c].validity, row);
-                    const int dt = B.cols[c].dtype;
-                    for (int k = L.col_kbegin[c]; k < L.col_kbegin[c + 1]; k++) {
-                        if (bulk_lane && k == L.pair_k) continue;      // already on its way as half of the bulk reduce
-                        gb_apply(L.wop[k], gb_wp(T, e, 2 + L.wslot[k]), dt, raw[c][r], valid, pol, hint);
-                    }
-                }
-            }
+            // bulk lanes: len and the paired sum are already on their way as the bulk reduce
+            gb_apply_row<MAXC>(L, T, B, e, row, [&](int c) { return raw[c][r]; }, pol, hint, bulk_lane);
         }
     }
     // all bulk reduces of this thread have been performed (not just read) before the CTA may retire
     if (BULK) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    // odd tail row
-    if ((B.n & 1) && blockIdx.x == 0 && threadIdx.x == 0) {
-        const int64_t row = B.n - 1;
-        bool kvalid = B.key_validity == nullptr || bit_get(B.key_validity, row);
-        uint64_t key = load_key_rt(B.keys, B.key_dtype, row);
-        const bool regular = kvalid && key != GB_EMPTY;
-        const bool mine = !T.pass_bits || (regular ? (int)(table_hash(key) >> (64 - T.pass_bits)) == T.pass_id : T.pass_id == 0);
-        uint64_t* e = !mine ? nullptr : (!kvalid ? gb_special(T, 0) : (key == GB_EMPTY ? gb_special(T, 1) : gb_find_or_insert(T, key)));
-        if (e) {
-            if (L.need_len) atomicAdd(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)), 1u);
-            if (L.need_first) atomicMin(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)) + 1, B.row_base + (uint32_t)row);
-            for (int c = 0; c < L.n_cols; c++) {
-                const bool valid = B.cols[c].validity == nullptr || bit_get(B.cols[c].validity, row);
-                uint64_t raw = B.cols[c].elem == 8 ? reinterpret_cast<const uint64_t*>(B.cols[c].values)[row] : (uint64_t)reinterpret_cast<const uint32_t*>(B.cols[c].values)[row];
-                for (int k = L.col_kbegin[c]; k < L.col_kbegin[c + 1]; k++) gb_apply(L.wop[k], gb_wp(T, e, 2 + L.wslot[k]), B.cols[c].dtype, raw, valid);
-            }
-        }
-    }
+    gb_tail_row(L, T, B);
 }
 
 // ---------------------------------------------------------------------------- K5, lean bulk-reduce kernel
@@ -320,23 +280,7 @@ __global__ void __launch_bounds__(256) k_gb_consume_lean(const __grid_constant__
             }
         }
     }
-    // odd tail row: plain atomics
-    if ((B.n & 1) && blockIdx.x == 0 && threadIdx.x == 0) {
-        const int64_t row = B.n - 1;
-        const uint64_t key = reinterpret_cast<const uint64_t*>(B.keys)[row];
-        const bool kvalid = B.key_validity == nullptr || bit_get(B.key_validity, row);
-        const bool regular = kvalid && key != GB_EMPTY;
-        const bool mine = !T.pass_bits || (regular ? (int)(table_hash(key) >> (64 - T.pass_bits)) == T.pass_id : T.pass_id == 0);
-        uint64_t* e = !mine ? nullptr : (!kvalid ? gb_special(T, 0) : (key == GB_EMPTY ? gb_special(T, 1) : gb_find_or_insert(T, key)));
-        if (e) {
-            atomicAdd(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)), 1u);
-            for (int c = 0; c < L.n_cols; c++) {
-                const uint64_t rv = reinterpret_cast<const uint64_t*>(B.cols[c].values)[row];
-                const bool valid = B.cols[c].validity == nullptr || bit_get(B.cols[c].validity, row);
-                for (int k = L.col_kbegin[c]; k < L.col_kbegin[c + 1]; k++) gb_apply(L.wop[k], gb_wp(T, e, 2 + L.wslot[k]), B.cols[c].dtype, rv, valid);
-            }
-        }
-    }
+    gb_tail_row(L, T, B);
     asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
@@ -414,15 +358,10 @@ __global__ void __launch_bounds__(256) k_gb_consume_hot(const __grid_constant__ 
         uint64_t kraw[2] = {0, 0};
         uint64_t raw[MAXC][2];
         if (in) {
-            if (KEY_ELEM == 8) { ulonglong2 t = ld_stream_u64x2(reinterpret_cast<const uint64_t*>(B.keys) + 2 * p); kraw[0] = t.x; kraw[1] = t.y; }
-            else { uint2 t = ld_stream_u32x2(reinterpret_cast<const uint32_t*>(B.keys) + 2 * p); kraw[0] = t.x; kraw[1] = t.y; }
+            gb_load_pair<KEY_ELEM>(B.keys, 2 * p, kraw[0], kraw[1]);
 #pragma unroll
-            for (int c = 0; c < MAXC; c++) {
-                if (c < L.n_cols) {
-                    if (B.cols[c].elem == 8) { ulonglong2 t = ld_stream_u64x2(reinterpret_cast<const uint64_t*>(B.cols[c].values) + 2 * p); raw[c][0] = t.x; raw[c][1] = t.y; }
-                    else { uint2 t = ld_stream_u32x2(reinterpret_cast<const uint32_t*>(B.cols[c].values) + 2 * p); raw[c][0] = t.x; raw[c][1] = t.y; }
-                }
-            }
+            for (int c = 0; c < MAXC; c++)
+                if (c < L.n_cols) gb_load_pair_rt(B.cols[c].values, B.cols[c].elem, 2 * p, raw[c][0], raw[c][1]);
         }
         uint64_t key[2], slot[2], k0[2];
         int kind[2], hidx[2];   // kind: 0 regular, 1 null-key group, 2 GB_EMPTY-key group, -1 no row;  hidx: accumulator row or -1 (cold)
@@ -488,38 +427,10 @@ __global__ void __launch_bounds__(256) k_gb_consume_hot(const __grid_constant__ 
         for (int r = 0; r < 2; r++) {
             if (kind[r] < 0 || hidx[r] >= 0) continue;
             uint64_t* e = kind[r] == 0 ? gb_resolve(T, key[r], slot[r], k0[r], 0, khint) : gb_special(T, kind[r] - 1);
-            if (e == nullptr) continue;
-            const int64_t row = 2 * p + r;
-            if (L.need_len) atomicAdd(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)), 1u);
-            if (L.need_first) atomicMin(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)) + 1, B.row_base + (uint32_t)row);
-#pragma unroll
-            for (int c = 0; c < MAXC; c++) {
-                if (c < L.n_cols) {
-                    const bool valid = B.cols[c].validity == nullptr || bit_get(B.cols[c].validity, row);
-                    const int dt = B.cols[c].dtype;
-                    for (int k = L.col_kbegin[c]; k < L.col_kbegin[c + 1]; k++) gb_apply(L.wop[k], gb_wp(T, e, 2 + L.wslot[k]), dt, raw[c][r], valid);
-                }
-            }
+            if (e) gb_apply_row<MAXC>(L, T, B, e, 2 * p + r, [&](int c) { return raw[c][r]; });
         }
     }
-    // odd tail row: straight to the global table
-    if ((B.n & 1) && blockIdx.x == 0 && threadIdx.x == 0) {
-        const int64_t row = B.n - 1;
-        bool kvalid = B.key_validity == nullptr || bit_get(B.key_validity, row);
-        uint64_t key = load_key_rt(B.keys, B.key_dtype, row);
-        const bool regular = kvalid && key != GB_EMPTY;
-        const bool mine = !T.pass_bits || (regular ? (int)(table_hash(key) >> (64 - T.pass_bits)) == T.pass_id : T.pass_id == 0);
-        uint64_t* e = !mine ? nullptr : (!kvalid ? gb_special(T, 0) : (key == GB_EMPTY ? gb_special(T, 1) : gb_find_or_insert(T, key)));
-        if (e) {
-            if (L.need_len) atomicAdd(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)), 1u);
-            if (L.need_first) atomicMin(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)) + 1, B.row_base + (uint32_t)row);
-            for (int c = 0; c < L.n_cols; c++) {
-                const bool valid = B.cols[c].validity == nullptr || bit_get(B.cols[c].validity, row);
-                uint64_t raw = B.cols[c].elem == 8 ? reinterpret_cast<const uint64_t*>(B.cols[c].values)[row] : (uint64_t)reinterpret_cast<const uint32_t*>(B.cols[c].values)[row];
-                for (int k = L.col_kbegin[c]; k < L.col_kbegin[c + 1]; k++) gb_apply(L.wop[k], gb_wp(T, e, 2 + L.wslot[k]), B.cols[c].dtype, raw, valid);
-            }
-        }
-    }
+    gb_tail_row(L, T, B);
     // merge the warp's accumulator rows into the global table (rows no lane touched keep len == 0)
     __syncwarp();
     for (int h = lane; h < H.rows; h += 32) {
@@ -669,16 +580,11 @@ __global__ void __launch_bounds__(512) k_gb_consume_smem(const __grid_constant__
     const int64_t gstride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < npairs; p += gstride) {
         uint64_t kraw[2];
-        if (KEY_ELEM == 8) { ulonglong2 t = ld_stream_u64x2(reinterpret_cast<const uint64_t*>(B.keys) + 2 * p); kraw[0] = t.x; kraw[1] = t.y; }
-        else { uint2 t = ld_stream_u32x2(reinterpret_cast<const uint32_t*>(B.keys) + 2 * p); kraw[0] = t.x; kraw[1] = t.y; }
+        gb_load_pair<KEY_ELEM>(B.keys, 2 * p, kraw[0], kraw[1]);
         uint64_t raw[MAXC][2];
 #pragma unroll
-        for (int c = 0; c < MAXC; c++) {
-            if (c < L.n_cols) {
-                if (FAST || B.cols[c].elem == 8) { ulonglong2 t = ld_stream_u64x2(reinterpret_cast<const uint64_t*>(B.cols[c].values) + 2 * p); raw[c][0] = t.x; raw[c][1] = t.y; }
-                else { uint2 t = ld_stream_u32x2(reinterpret_cast<const uint32_t*>(B.cols[c].values) + 2 * p); raw[c][0] = t.x; raw[c][1] = t.y; }
-            }
-        }
+        for (int c = 0; c < MAXC; c++)
+            if (c < L.n_cols) gb_load_pair_rt(B.cols[c].values, FAST ? 8 : B.cols[c].elem, 2 * p, raw[c][0], raw[c][1]);
 #pragma unroll
         for (int j = 0; j < 2; j++) {
             const int64_t row = 2 * p + j;
@@ -717,37 +623,11 @@ __global__ void __launch_bounds__(512) k_gb_consume_smem(const __grid_constant__
                 }
             } else {
                 uint64_t* e = gb_find_or_insert(T, key);
-                if (e != nullptr) {
-                    if (L.need_len) atomicAdd(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)), 1u);
-                    if (L.need_first) atomicMin(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)) + 1, B.row_base + (uint32_t)row);
-#pragma unroll
-                    for (int c = 0; c < MAXC; c++) {
-                        if (c < L.n_cols) {
-                            const bool valid = B.cols[c].validity == nullptr || bit_get(B.cols[c].validity, row);
-                            const int dt = B.cols[c].dtype;
-                            for (int k = L.col_kbegin[c]; k < L.col_kbegin[c + 1]; k++) gb_apply(L.wop[k], gb_wp(T, e, 2 + L.wslot[k]), dt, raw[c][j], valid);
-                        }
-                    }
-                }
+                if (e != nullptr) gb_apply_row<MAXC>(L, T, B, e, row, [&](int c) { return raw[c][j]; });
             }
         }
     }
-    // odd tail row: straight to the global table
-    if ((B.n & 1) && blockIdx.x == 0 && threadIdx.x == 0) {
-        const int64_t row = B.n - 1;
-        bool kvalid = B.key_validity == nullptr || bit_get(B.key_validity, row);
-        uint64_t key = load_key_rt(B.keys, B.key_dtype, row);
-        uint64_t* e = !kvalid ? gb_special(T, 0) : (key == GB_EMPTY ? gb_special(T, 1) : gb_find_or_insert(T, key));
-        if (e) {
-            if (L.need_len) atomicAdd(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)), 1u);
-            if (L.need_first) atomicMin(reinterpret_cast<unsigned*>(gb_wp(T, e, 1)) + 1, B.row_base + (uint32_t)row);
-            for (int c = 0; c < L.n_cols; c++) {
-                const bool valid = B.cols[c].validity == nullptr || bit_get(B.cols[c].validity, row);
-                uint64_t raw = B.cols[c].elem == 8 ? reinterpret_cast<const uint64_t*>(B.cols[c].values)[row] : (uint64_t)reinterpret_cast<const uint32_t*>(B.cols[c].values)[row];
-                for (int k = L.col_kbegin[c]; k < L.col_kbegin[c + 1]; k++) gb_apply(L.wop[k], gb_wp(T, e, 2 + L.wslot[k]), B.cols[c].dtype, raw, valid);
-            }
-        }
-    }
+    gb_tail_row(L, T, B);      // launched with pass_bits == 0: every row is this launch's
     __syncthreads();
     // merge the CTA's partial aggregates into the global table
     for (int i = threadIdx.x; i < copies * n_ent; i += blockDim.x) {
@@ -868,15 +748,6 @@ __global__ void __launch_bounds__(256) k_gb_finalize_all(const __grid_constant__
     }
 }
 
-// typed key column from u64 key bits (+ validity with the null group cleared)
-__global__ void k_gb_keys_out(const uint64_t* bits, int64_t G, int elem, void* out, uint32_t* out_valid, long long null_pos) {
-    const int64_t rounded = (G + 31) / 32 * 32;
-    for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < rounded; g += (int64_t)gridDim.x * blockDim.x) {
-        if (g < G) { if (elem == 8) reinterpret_cast<uint64_t*>(out)[g] = bits[g]; else reinterpret_cast<uint32_t*>(out)[g] = (uint32_t)bits[g]; }
-        if (out_valid) { unsigned b = __ballot_sync(0xffffffffu, g < G && g != null_pos); if (lane_id() == 0) out_valid[g >> 5] = b; }
-    }
-}
-
 // ---------------------------------------------------------------------------- K6: partitioned export of partial rows
 // row = [key, len|first, words..., meta]; partition = hash_to_partition(dirty_hash(key), P), null-key group -> 0.
 // Block-local reservation: smem histogram -> one global atomicAdd per (block, partition) -> smem cursors.
@@ -896,41 +767,20 @@ __global__ void __launch_bounds__(256) k_gb_export_count(const uint64_t* __restr
     __syncthreads();
     if (threadIdx.x < P && hist[threadIdx.x]) atomicAdd(&part_counts[threadIdx.x], (unsigned long long)hist[threadIdx.x]);
 }
-__global__ void __launch_bounds__(256) k_gb_export_scatter(const uint64_t* __restrict__ entries, int64_t cap, int64_t es, int64_t ws, int pw, int n_words, int P,
-                                                           const unsigned long long* __restrict__ part_off, unsigned long long* part_cursor, uint64_t* __restrict__ rows) {
-    __shared__ unsigned hist[EXP_MAX_PARTS];
-    __shared__ unsigned long long base[EXP_MAX_PARTS];
-    const int row_words = n_words + 3;
-    const int64_t n_entries = cap + 2;
-    const int64_t ntiles = (n_entries + 255) / 256;
-    for (int64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        if (threadIdx.x < EXP_MAX_PARTS) hist[threadIdx.x] = 0;
-        __syncthreads();
-        const int64_t s = t * 256 + threadIdx.x;
-        uint64_t key = GB_EMPTY; int p = 0; unsigned local = 0;
-        if (s < n_entries) key = entries[s * es];
-        if (key != GB_EMPTY) { p = gb_row_partition(key, s, cap, P); local = atomicAdd(&hist[p], 1u); }
-        __syncthreads();
-        if (threadIdx.x < P && hist[threadIdx.x]) base[threadIdx.x] = part_off[threadIdx.x] + atomicAdd(&part_cursor[threadIdx.x], (unsigned long long)hist[threadIdx.x]);
-        __syncthreads();
-        if (key != GB_EMPTY) {
-            const uint64_t* e = entries + s * es;
-            uint64_t* dst = rows + (base[p] + local) * row_words;
-            dst[0] = s == cap ? 0 : (s == cap + 1 ? GB_EMPTY : key);
-            dst[1] = e[gb_woff(s, 1, ws, pw)];
-            for (int w = 0; w < n_words; w++) dst[2 + w] = e[gb_woff(s, 2 + w, ws, pw)];
-            dst[2 + n_words] = s == cap ? 1 : (s == cap + 1 ? 2 : 0);
-        }
-        __syncthreads();
-    }
+// the partial row of used slot s (key word `key`) at dst
+__device__ __forceinline__ void gb_export_row(uint64_t* dst, const uint64_t* __restrict__ entries, int64_t s, uint64_t key, int64_t cap, int64_t es, int64_t ws, int pw, int n_words) {
+    const uint64_t* e = entries + s * es;
+    dst[0] = s == cap ? 0 : (s == cap + 1 ? GB_EMPTY : key);
+    dst[1] = e[gb_woff(s, 1, ws, pw)];
+    for (int w = 0; w < n_words; w++) dst[2 + w] = e[gb_woff(s, 2 + w, ws, pw)];
+    dst[2 + n_words] = s == cap ? 1 : (s == cap + 1 ? 2 : 0);
 }
-
-// Fused partition + exchange: same block-local reservation as k_gb_export_scatter, but the row is
-// stored straight into the destination rank's window (peer memory over NVLink): partition p's rows
-// land in region `my_rank` of windows[p] at [cursor .. cursor + n).  No staging copy, no collective.
-struct PeerWindows { uint64_t* base[EXP_MAX_PARTS]; };
-__global__ void __launch_bounds__(256) k_gb_export_p2p(const uint64_t* __restrict__ entries, int64_t cap, int64_t es, int64_t ws, int pw, int n_words, int P, const __grid_constant__ PeerWindows W,
-                                                       int64_t region_words, int my_rank, int64_t rows_per_src, unsigned long long* part_cursor, int* overflow) {
+// Partition p's rows go to D.base[p] + [cursor .. cursor + n) rows: a region of the local export buffer, or region
+// `my_rank` of rank p's window (peer memory over NVLink: partition and exchange in one kernel, no staging copy, no
+// collective).  Rows at or past `limit` in their partition are not stored and set *overflow.
+struct PartDst { uint64_t* base[EXP_MAX_PARTS]; };
+__global__ void __launch_bounds__(256) k_gb_export_scatter(const uint64_t* __restrict__ entries, int64_t cap, int64_t es, int64_t ws, int pw, int n_words, int P, const __grid_constant__ PartDst D,
+                                                           int64_t limit, unsigned long long* part_cursor, int* overflow) {
     __shared__ unsigned hist[EXP_MAX_PARTS];
     __shared__ unsigned long long base[EXP_MAX_PARTS];
     const int row_words = n_words + 3;
@@ -948,15 +798,8 @@ __global__ void __launch_bounds__(256) k_gb_export_p2p(const uint64_t* __restric
         __syncthreads();
         if (key != GB_EMPTY) {
             const uint64_t pos = base[p] + local;
-            if ((int64_t)pos >= rows_per_src) *overflow = 1;
-            else {
-                const uint64_t* e = entries + s * es;
-                uint64_t* dst = W.base[p] + (int64_t)my_rank * region_words + pos * row_words;     // peer store
-                dst[0] = s == cap ? 0 : (s == cap + 1 ? GB_EMPTY : key);
-                dst[1] = e[gb_woff(s, 1, ws, pw)];
-                for (int w = 0; w < n_words; w++) dst[2 + w] = e[gb_woff(s, 2 + w, ws, pw)];
-                dst[2 + n_words] = s == cap ? 1 : (s == cap + 1 ? 2 : 0);
-            }
+            if ((int64_t)pos >= limit) *overflow = 1;
+            else gb_export_row(D.base[p] + pos * row_words, entries, s, key, cap, es, ws, pw, n_words);
         }
         __syncthreads();
     }
@@ -974,7 +817,7 @@ __device__ __forceinline__ void st_release_sys_u64(uint64_t* p, uint64_t v) { as
 __device__ __forceinline__ uint64_t ld_acquire_sys_u64(const uint64_t* p) { uint64_t v; asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory"); return v; }
 constexpr unsigned long long GB_WINDOW_OVERFLOW = ~0ull;
 
-__global__ void __launch_bounds__(256) k_gb_export_p2p_async(const uint64_t* __restrict__ entries, int64_t cap, int64_t es, int64_t ws, int pw, int n_words, int P, const __grid_constant__ PeerWindows W,
+__global__ void __launch_bounds__(256) k_gb_export_p2p_async(const uint64_t* __restrict__ entries, int64_t cap, int64_t es, int64_t ws, int pw, int n_words, int P, const __grid_constant__ PartDst W,
                                                              int64_t region_words, int my_rank, int64_t rows_per_src, unsigned long long* part_cursor, unsigned* done, uint64_t epoch) {
     __shared__ unsigned hist[EXP_MAX_PARTS];
     __shared__ unsigned long long base[EXP_MAX_PARTS];
@@ -1006,14 +849,8 @@ __global__ void __launch_bounds__(256) k_gb_export_p2p_async(const uint64_t* __r
             if (key[u] == GB_EMPTY) continue;
             const int64_t s = t * TILE + u * 256 + threadIdx.x;
             const uint64_t pos = base[p[u]] + local[u];
-            if ((int64_t)pos < rows_per_src) {
-                const uint64_t* e = entries + s * es;
-                uint64_t* dst = W.base[p[u]] + GB_WINDOW_HEADER_WORDS + (int64_t)my_rank * region_words + pos * row_words;     // peer store
-                dst[0] = s == cap ? 0 : (s == cap + 1 ? GB_EMPTY : key[u]);
-                dst[1] = e[gb_woff(s, 1, ws, pw)];
-                for (int w = 0; w < n_words; w++) dst[2 + w] = e[gb_woff(s, 2 + w, ws, pw)];
-                dst[2 + n_words] = s == cap ? 1 : (s == cap + 1 ? 2 : 0);
-            }
+            if ((int64_t)pos < rows_per_src)      // peer store
+                gb_export_row(W.base[p[u]] + GB_WINDOW_HEADER_WORDS + (int64_t)my_rank * region_words + pos * row_words, entries, s, key[u], cap, es, ws, pw, n_words);
         }
         __syncthreads();
     }
@@ -1077,8 +914,6 @@ __global__ void __launch_bounds__(256) k_gb_merge_window(const __grid_constant__
 // =============================================================================================
 namespace plb {
 
-static int knob_int(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }   // read per call (tests flip them)
-
 static int sum_out_dtype(int dt) {
     // series/implementations/mod.rs:145-154: Int8/16, UInt8/16 sums are computed as Int64
     if (dt == BL_INT8 || dt == BL_INT16 || dt == BL_UINT8 || dt == BL_UINT16) return BL_INT64;
@@ -1126,9 +961,9 @@ void GroupByState::alloc_table(uint64_t new_cap) {
     cap = new_cap;
     entries = dev_alloc((size_t)(cap + 2) * L.stride * 8);
     int shift = 64; for (uint64_t c = cap; c > 1; c >>= 1) shift--;
-    const int hint = [] { const char* e = getenv("BL_K5_HINT"); return e ? atoi(e) : 0; }();
+    const int hint = knob_int("BL_K5_HINT", 0);
     // word-major planes by default: the REDs of one row then hit different sectors / L2 slices (ubench: 54 vs 38 G rows/s)
-    const int soa = [] { const char* e = getenv("BL_K5_SOA"); return e ? atoi(e) : 1; }();
+    const int soa = knob_int("BL_K5_SOA", 1);
     T.entries = as<uint64_t>(entries); T.cap = cap; T.shift = shift; T.status = as<int>(status); T.hint = hint;
     T.es = soa ? 1 : L.stride; T.ws = soa ? (int64_t)(cap + 2) : 1; T.soa = soa; T.pass_bits = 0; T.pass_id = 0;
     // pair layout + bulk reduce (k_gb_consume<BULK>): only where the plain-RED kernels do not run on this table — the shared-memory plan
@@ -1137,9 +972,7 @@ void GroupByState::alloc_table(uint64_t new_cap) {
     // the GENERAL bulk kernel is issue-bound and loses, most with nulls); 2 always (parity tests of the general kernel)
     const int bulk_knob = knob_int("BL_K5_BULK", 1);
     const int bulk = bulk_knob >= 2 ? 1 : (bulk_knob == 1 && lean_shape ? 1 : 0);
-    bool smem_plan = false;     // same rule as launch_batch
-    if (est_groups > 0 && knob_int("BL_K5_SMEM", 1)) { int64_t want = 16; while (2 * want < 3 * est_groups && want < (1 << 20)) want <<= 1; smem_plan = (size_t)(want + 2) * L.stride * 8 <= (size_t)72 * 1024; }
-    T.pw = (soa && bulk > 0 && pair_word >= 2 && hot.rows == 0 && !smem_plan) ? pair_word : 0;
+    T.pw = (soa && bulk > 0 && pair_word >= 2 && hot.rows == 0 && !smem_table_cap()) ? pair_word : 0;
     T.bulk_lanes = T.pw ? std::min(32, std::max(0, knob_int("BL_K5_BULK_LANES", 32))) : 0;
     PLB_LAUNCH("k5_table_init", k_gb_init, grid_for((int64_t)(cap + 2) * L.stride, 256), 256, 0, T.entries, (int64_t)(cap + 2), L.stride, soa, T.pw, L);
     dev_memset(status->p, 0, 4);
@@ -1160,8 +993,7 @@ static double estimate_groups(double d, double m, double n) {
 void GroupByState::build_hot_list(const void* cand_v, int n_cand, bool null_hot, bool empty_hot, double m) {
     const GbCandidate* cand = static_cast<const GbCandidate*>(cand_v);
     hot = GbHotDev{}; hot_share = 0; hot_buf.reset();
-    const int on = [] { const char* e = getenv("BL_K5_HOTKEYS"); return e ? atoi(e) : 1; }();
-    if (!on || (n_cand <= 0 && !null_hot && !empty_hot)) return;
+    if (!knob_int("BL_K5_HOTKEYS", 1) || (n_cand <= 0 && !null_hot && !empty_hot)) return;
     std::vector<GbCandidate> c(cand, cand + std::max(n_cand, 0));
     std::sort(c.begin(), c.end(), [](const GbCandidate& a, const GbCandidate& b) { return a.mult > b.mult || (a.mult == b.mult && a.key < b.key); });
     const int row_words = 2 + L.n_words;
@@ -1197,7 +1029,7 @@ uint64_t GroupByState::choose_cap(const DevCol& key, int64_t n_total) {
         GbCandidate* dcand = reinterpret_cast<GbCandidate*>(dstats + 1);
         const double nt = (double)std::max<int64_t>(n_total, n);
         // a key is "hot" when its rows would serialise on one L2 address for >~0.15 ms (a few ns per same-address RED)
-        const double hot_rows = [] { const char* e = getenv("BL_K5_HOT_ROWS"); double v = e ? atof(e) : 30000.0; return v >= 0 ? v : 30000.0; }();
+        const double hot_knob = knob_double("BL_K5_HOT_ROWS", 30000.0), hot_rows = hot_knob >= 0 ? hot_knob : 30000.0;
         const unsigned hot_thr = (unsigned)std::max(12.0, std::ceil(hot_rows * (double)m / nt));
         PLB_LAUNCH("k5_fill", k_fill_u64, grid_for(scap, 256), 256, 0, as<uint64_t>(scratch), GB_EMPTY, (int64_t)scap);
         dev_memset(mult->p, 0, scap * 4 + sizeof(GbSampleStats));
@@ -1238,7 +1070,7 @@ uint64_t GroupByState::choose_cap(const DevCol& key, int64_t n_total) {
         build_hot_list(cand, (int)std::min<unsigned>(st.n_cand, GB_CAND_MAX), st.nulls >= hot_thr, st.empties >= hot_thr, (double)m);
     }
     est_groups = (int64_t)(G_raw * 1.25) + 2;      // for the shared-memory plan (overflow falls through to the global table)
-    const double lf = [] { const char* e = getenv("BL_K5_LF"); double v = e ? atof(e) / 100.0 : 0.6; return (v > 0.05 && v < 0.95) ? v : 0.6; }();
+    const double lf_knob = knob_double("BL_K5_LF", 60.0) / 100.0, lf = (lf_knob > 0.05 && lf_knob < 0.95) ? lf_knob : 0.6;
     uint64_t c = pow2_at_least(G / lf);       // load factor <= 0.6 by default
     // keep the table inside L2 when a load factor <= 0.85 allows it: past ~55 % of L2 the REDs miss and the
     // kernel slows down ~3x, while linear probing over
@@ -1256,11 +1088,11 @@ uint64_t GroupByState::choose_cap(const DevCol& key, int64_t n_total) {
 
 template <int KEY_ELEM, int KEY_CANON, bool KEY_NULLS, int PAIRS, bool BULK>
 static void launch_consume_p(const GbLayout& L, const GbTableDev& T, const GbBatch& B, int grid) {
-    const size_t smem = BULK ? (size_t)2 * PAIRS * 256 * 16 : 0;     // staging cells of the bulk reduces
-    if (L.n_cols <= 1) PLB_LAUNCH("k5_groupby_agg", (k_gb_consume<KEY_ELEM, KEY_CANON, KEY_NULLS, 1, PAIRS, BULK>), grid, 256, smem, L, T, B);
-    else if (L.n_cols <= 2) PLB_LAUNCH("k5_groupby_agg", (k_gb_consume<KEY_ELEM, KEY_CANON, KEY_NULLS, 2, PAIRS, BULK>), grid, 256, smem, L, T, B);
-    else if (L.n_cols <= 4) PLB_LAUNCH("k5_groupby_agg", (k_gb_consume<KEY_ELEM, KEY_CANON, KEY_NULLS, 4, PAIRS, BULK>), grid, 256, smem, L, T, B);
-    else PLB_LAUNCH("k5_groupby_agg", (k_gb_consume<KEY_ELEM, KEY_CANON, KEY_NULLS, 8, 1, BULK>), grid, 256, BULK ? (size_t)2 * 256 * 16 : 0, L, T, B);
+    with_at_least<1, 2, 4, 8>(L.n_cols, [&](auto maxc) {
+        constexpr int MAXC = decltype(maxc)::value, P = MAXC == 8 ? 1 : PAIRS;     // 8 columns: one row pair per thread
+        const size_t smem = BULK ? (size_t)2 * P * 256 * 16 : 0;     // staging cells of the bulk reduces
+        PLB_LAUNCH("k5_groupby_agg", (k_gb_consume<KEY_ELEM, KEY_CANON, KEY_NULLS, MAXC, P, BULK>), grid, 256, smem, L, T, B);
+    });
 }
 template <int KEY_ELEM, int KEY_CANON, bool KEY_NULLS>
 static void launch_consume(const GbLayout& L, const GbTableDev& T, const GbBatch& B, int grid) {
@@ -1271,69 +1103,64 @@ static void launch_consume(const GbLayout& L, const GbTableDev& T, const GbBatch
                     knob_int("BL_K5_LEAN", 1) != 0;
         bool nulls = KEY_NULLS;
         for (int c = 0; lean && c < L.n_cols; c++) { lean = B.cols[c].elem == 8 && L.col_kbegin[c + 1] - L.col_kbegin[c] <= 2; nulls = nulls || B.cols[c].validity != nullptr; }
-        if (lean) {
-            const size_t smem = (size_t)2 * 256 * 16;
-#define GB_LEAN(NC) do { if (nulls) PLB_LAUNCH("k5_groupby_agg", (k_gb_consume_lean<NC, true>), grid, 256, smem, L, T, B); \
-                         else PLB_LAUNCH("k5_groupby_agg", (k_gb_consume_lean<NC, false>), grid, 256, smem, L, T, B); } while (0)
-            if (L.n_cols == 1) GB_LEAN(1); else if (L.n_cols == 2) GB_LEAN(2); else GB_LEAN(3);
-#undef GB_LEAN
-        } else launch_consume_p<KEY_ELEM, KEY_CANON, KEY_NULLS, 1, true>(L, T, B, grid);
+        if (lean) with_at_least<1, 2, 3>(L.n_cols, [&](auto nc) { with_bool(nulls, [&](auto nl) {
+            PLB_LAUNCH("k5_groupby_agg", (k_gb_consume_lean<decltype(nc)::value, decltype(nl)::value>), grid, 256, (size_t)2 * 256 * 16, L, T, B);
+        }); });
+        else launch_consume_p<KEY_ELEM, KEY_CANON, KEY_NULLS, 1, true>(L, T, B, grid);
     }
     else if (pairs == 2) launch_consume_p<KEY_ELEM, KEY_CANON, KEY_NULLS, 2, false>(L, T, B, grid);
     else launch_consume_p<KEY_ELEM, KEY_CANON, KEY_NULLS, 1, false>(L, T, B, grid);
 }
 
-template <int KEY_ELEM, int KEY_CANON, bool KEY_NULLS, int MAXC>
-static void launch_hot_c(const GbLayout& L, const GbTableDev& T, const GbBatch& B, const GbHotDev& H, int grid) {
-    auto kfn = k_gb_consume_hot<KEY_ELEM, KEY_CANON, KEY_NULLS, MAXC>;
-    const size_t smem = (size_t)GB_HOT_SLOTS * 8 + (size_t)8 * H.rows * (2 + L.n_words) * 8 + GB_HOT_SLOTS;
-    PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    PLB_LAUNCH("k5_groupby_agg_hot", kfn, grid, 256, smem, L, T, B, H);
-}
 template <int KEY_ELEM, int KEY_CANON, bool KEY_NULLS>
 static void launch_hot(const GbLayout& L, const GbTableDev& T, const GbBatch& B, const GbHotDev& H, int grid) {
-    if (L.n_cols <= 1) launch_hot_c<KEY_ELEM, KEY_CANON, KEY_NULLS, 1>(L, T, B, H, grid);
-    else if (L.n_cols <= 2) launch_hot_c<KEY_ELEM, KEY_CANON, KEY_NULLS, 2>(L, T, B, H, grid);
-    else if (L.n_cols <= 4) launch_hot_c<KEY_ELEM, KEY_CANON, KEY_NULLS, 4>(L, T, B, H, grid);
-    else launch_hot_c<KEY_ELEM, KEY_CANON, KEY_NULLS, 8>(L, T, B, H, grid);
+    with_at_least<1, 2, 4, 8>(L.n_cols, [&](auto maxc) {
+        auto kfn = k_gb_consume_hot<KEY_ELEM, KEY_CANON, KEY_NULLS, decltype(maxc)::value>;
+        const size_t smem = (size_t)GB_HOT_SLOTS * 8 + (size_t)8 * H.rows * (2 + L.n_words) * 8 + GB_HOT_SLOTS;
+        PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PLB_LAUNCH("k5_groupby_agg_hot", kfn, grid, 256, smem, L, T, B, H);
+    });
 }
 
-template <int KEY_ELEM, int KEY_CANON, bool KEY_NULLS, int MAXC, bool FAST>
-static void launch_smem_cf(const GbLayout& L, const GbTableDev& T, const GbBatch& B, int scap) {
-    auto kfn = k_gb_consume_smem<KEY_ELEM, KEY_CANON, KEY_NULLS, MAXC, FAST>;
-    const size_t tab_bytes = ((size_t)(scap + 2) * L.stride + 2) * 8;
-    const int copies = (int)std::min<size_t>(32, std::max<size_t>(1, (size_t)(96 * 1024) / tab_bytes));
-    const size_t smem = tab_bytes * copies;
-    PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = (int)std::min<size_t>(4, std::max<size_t>(1, (size_t)(220 * 1024) / (smem + 1024)));
-    int sshift = 64; for (int c = scap; c > 1; c >>= 1) sshift--;
-    const int grid = (int)std::min<int64_t>((int64_t)ctx().sm_count * per_sm, std::max<int64_t>(1, (B.n / 2 + 511) / 512));
-    PLB_LAUNCH("k5_groupby_agg_smem", kfn, grid, 512, smem, L, T, B, scap, sshift, copies);
+// shared-memory plan: CTA-private tables of this many slots (0: the estimated groups do not fit one)
+int GroupByState::smem_table_cap() const {
+    if (est_groups <= 0 || !knob_int("BL_K5_SMEM", 1)) return 0;
+    // load factor <= 2/3 (probing a shared-memory table is cheap; occupancy is not)
+    int want = 16; while (2 * want < 3 * est_groups && want < (1 << 20)) want <<= 1;   // tiny tables leave room for up to 32 replicas
+    // beyond ~72 KB of table per CTA the occupancy loss outweighs the cheaper atomics
+    return (size_t)(want + 2) * L.stride * 8 <= (size_t)72 * 1024 ? want : 0;
 }
-template <int KEY_ELEM, int KEY_CANON, bool KEY_NULLS, int MAXC>
-static void launch_smem_c(const GbLayout& L, const GbTableDev& T, const GbBatch& B, int scap) {
-    bool fast = true;
-    for (int c = 0; c < L.n_cols; c++) fast = fast && B.cols[c].elem == 8 && B.cols[c].validity == nullptr;
-    if (fast) launch_smem_cf<KEY_ELEM, KEY_CANON, KEY_NULLS, MAXC, true>(L, T, B, scap);
-    else launch_smem_cf<KEY_ELEM, KEY_CANON, KEY_NULLS, MAXC, false>(L, T, B, scap);
-}
+static size_t smem_table_bytes(int scap, int stride) { return ((size_t)(scap + 2) * stride + 2) * 8; }
+// replicas of the shared-memory table in one CTA: as many as fit 96 KB, 1 to 32
+static int smem_copies(int scap, int stride) { return (int)std::min<size_t>(32, std::max<size_t>(1, (size_t)(96 * 1024) / smem_table_bytes(scap, stride))); }
+
 template <int KEY_ELEM, int KEY_CANON, bool KEY_NULLS>
 static void launch_smem(const GbLayout& L, const GbTableDev& T, const GbBatch& B, int scap) {
-    if (L.n_cols <= 1) launch_smem_c<KEY_ELEM, KEY_CANON, KEY_NULLS, 1>(L, T, B, scap);
-    else if (L.n_cols <= 2) launch_smem_c<KEY_ELEM, KEY_CANON, KEY_NULLS, 2>(L, T, B, scap);
-    else if (L.n_cols <= 4) launch_smem_c<KEY_ELEM, KEY_CANON, KEY_NULLS, 4>(L, T, B, scap);
-    else launch_smem_c<KEY_ELEM, KEY_CANON, KEY_NULLS, 8>(L, T, B, scap);
+    bool fast = true;
+    for (int c = 0; c < L.n_cols; c++) fast = fast && B.cols[c].elem == 8 && B.cols[c].validity == nullptr;
+    with_at_least<1, 2, 4, 8>(L.n_cols, [&](auto maxc) { with_bool(fast, [&](auto f) {
+        auto kfn = k_gb_consume_smem<KEY_ELEM, KEY_CANON, KEY_NULLS, decltype(maxc)::value, decltype(f)::value>;
+        const int copies = smem_copies(scap, L.stride);
+        const size_t smem = smem_table_bytes(scap, L.stride) * copies;
+        PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int per_sm = (int)std::min<size_t>(4, std::max<size_t>(1, (size_t)(220 * 1024) / (smem + 1024)));
+        int sshift = 64; for (int c = scap; c > 1; c >>= 1) sshift--;
+        const int grid = (int)std::min<int64_t>((int64_t)ctx().sm_count * per_sm, std::max<int64_t>(1, (B.n / 2 + 511) / 512));
+        PLB_LAUNCH("k5_groupby_agg_smem", kfn, grid, 512, smem, L, T, B, scap, sshift, copies);
+    }); });
 }
 
-void GroupByState::launch_batch(const DevCol& key, const std::vector<const DevCol*>& values, int64_t row_base) {
-    // per-batch column binding: aggregations over the same buffer share one column slot
-    GbBatch B; memset(&B, 0, sizeof B);
+// Per-batch column binding: aggregations over the same buffer share one column slot; col_kbegin / wslot / wop list each
+// column's accumulator words, null counters only where the column carries a validity bitmap.  pw != 0 (pair layout): the
+// column of the paired integer sum is bound first (column 0: the bulk-reduce kernels read it with a static index) and
+// pair_k is set.  false: more than max_cols distinct value columns.
+bool GroupByState::bind_columns(const DevCol& key, const std::vector<const DevCol*>& values, int64_t row_base, int pw, int max_cols, GbBatch& B, GbLayout& Lb) const {
+    memset(&B, 0, sizeof B);
     B.keys = key.v(); B.key_validity = key.vm(); B.n = key.len; B.row_base = (uint32_t)row_base; B.key_dtype = key.dtype;
     std::vector<const void*> col_ptr; std::vector<int> col_of_agg(plans.size(), -1);
-    // pair layout: the column of the paired integer sum is bound first (column 0: the bulk-reduce kernel reads it with a static index)
     std::vector<size_t> plan_order;
-    for (size_t i = 0; i < plans.size(); i++) if (T.pw && plans[i].main == T.pw - 2) plan_order.push_back(i);
-    for (size_t i = 0; i < plans.size(); i++) if (!(T.pw && plans[i].main == T.pw - 2)) plan_order.push_back(i);
+    for (size_t i = 0; i < plans.size(); i++) if (pw && plans[i].main == pw - 2) plan_order.push_back(i);
+    for (size_t i = 0; i < plans.size(); i++) if (!(pw && plans[i].main == pw - 2)) plan_order.push_back(i);
     for (size_t i : plan_order) {
         if (plans[i].kind == BL_AGG_LEN) continue;
         const DevCol* v = values[i];
@@ -1343,13 +1170,13 @@ void GroupByState::launch_batch(const DevCol& key, const std::vector<const DevCo
         int c = -1;
         for (size_t j = 0; j < col_ptr.size(); j++) if (col_ptr[j] == v->v() && B.cols[j].validity == v->vm()) c = (int)j;
         if (c < 0) {
-            PLB_REQUIRE(col_ptr.size() < GB_MAX_COLS, BL_ERR_UNSUPPORTED, "group_by: more than 8 distinct value columns in one pass");
+            if ((int)col_ptr.size() >= max_cols) return false;
             c = (int)col_ptr.size(); col_ptr.push_back(v->v());
             B.cols[c].values = v->v(); B.cols[c].validity = v->vm(); B.cols[c].dtype = v->dtype; B.cols[c].elem = dtype_size(v->dtype);
         }
         col_of_agg[i] = c;
     }
-    GbLayout Lb = L;
+    Lb = L;
     Lb.n_cols = (int)col_ptr.size();
     int k = 0;
     for (int c = 0; c < Lb.n_cols; c++) {
@@ -1357,13 +1184,18 @@ void GroupByState::launch_batch(const DevCol& key, const std::vector<const DevCo
         for (size_t i = 0; i < plans.size(); i++) {
             if (col_of_agg[i] != c) continue;
             if (plans[i].main >= 0) { Lb.wslot[k] = plans[i].main; Lb.wop[k] = L.slot_op[plans[i].main]; k++; }
-            // null counters only matter when the column can hold nulls
             if (plans[i].nullcnt >= 0 && B.cols[c].validity != nullptr) { Lb.wslot[k] = plans[i].nullcnt; Lb.wop[k] = W_NULLCNT; k++; }
         }
     }
     for (int c = Lb.n_cols; c <= GB_MAX_COLS; c++) Lb.col_kbegin[c] = k;
     Lb.pair_k = -1; Lb.pair_c = -1;
-    if (T.pw) for (int c = 0; c < Lb.n_cols; c++) for (int j = Lb.col_kbegin[c]; j < Lb.col_kbegin[c + 1]; j++) if (c == 0 && 2 + Lb.wslot[j] == T.pw && Lb.wop[j] == W_ADD_INT) { Lb.pair_k = j; Lb.pair_c = c; }
+    if (pw) for (int j = Lb.col_kbegin[0]; j < Lb.col_kbegin[1]; j++) if (2 + Lb.wslot[j] == pw && Lb.wop[j] == W_ADD_INT) { Lb.pair_k = j; Lb.pair_c = 0; }
+    return true;
+}
+
+void GroupByState::launch_batch(const DevCol& key, const std::vector<const DevCol*>& values, int64_t row_base) {
+    GbBatch B; GbLayout Lb;
+    PLB_REQUIRE(bind_columns(key, values, row_base, T.pw, GB_MAX_COLS, B, Lb), BL_ERR_UNSUPPORTED, "group_by: more than 8 distinct value columns in one pass");
     const int64_t n = key.len;
     if (n == 0) return;
     // CTAs per SM of the grid-stride launch (more than are resident: 5-6; shorter CTAs even out the tail).  BL_K5_BPS overrides.
@@ -1371,55 +1203,40 @@ void GroupByState::launch_batch(const DevCol& key, const std::vector<const DevCo
     const int bps = std::max(1, knob_int("BL_K5_BPS", lean_table ? 48 : 24));
     const int grid = grid_for((n / 2 + 1), 256, bps);
     const int grid_hot = grid_for((n / 2 + 1), 256, std::max(1, knob_int("BL_K5_BPS", 8)));     // every warp merges its private rows at the end: keep the CTA count low
-    const bool kn = key.validity != nullptr;
-    const int elem = dtype_size(key.dtype);
-    const int canon = key.dtype == BL_FLOAT64 ? 1 : (key.dtype == BL_FLOAT32 ? 2 : 0);
     // keys must be 16-byte aligned for the 128-bit path (device columns always are)
     // low-cardinality plan: CTA-private shared-memory tables (largest table that leaves >= 1 CTA per SM)
-    const int smem_on = [] { const char* e = getenv("BL_K5_SMEM"); return e ? atoi(e) : 1; }();
-    int scap = 0;
-    if (smem_on && est_groups > 0) {
-        // load factor <= 2/3 (probing a shared-memory table is cheap; occupancy is not)
-        int want = 16; while (2 * want < 3 * est_groups && want < (1 << 20)) want <<= 1;   // tiny tables leave room for up to 32 replicas
-        // beyond ~72 KB of table per CTA the occupancy loss outweighs the cheaper atomics
-        if ((size_t)(want + 2) * Lb.stride * 8 <= (size_t)72 * 1024) scap = want;
-    }
+    int scap = smem_table_cap();
     // skewed keys: the CTA-private tables serialise on the hot key's shared-memory address as soon as more than a
     // few of the CTA's 512 threads work on it; with too few replicas to spread
     // that load, take the global table + warp-private heavy-hitter rows instead
-    if (scap && hot.rows > 0) {
-        const size_t tab_bytes = ((size_t)(scap + 2) * Lb.stride + 2) * 8;
-        const double copies = (double)std::min<size_t>(32, std::max<size_t>(1, (size_t)(96 * 1024) / tab_bytes));
-        if (hot_share * 512.0 / copies > 4.0) scap = 0;
-    }
+    if (scap && hot.rows > 0 && hot_share * 512.0 / (double)smem_copies(scap, Lb.stride) > 4.0) scap = 0;
     // hot-table mode (experimental knob): run the shared-memory kernel with BL_K5_HOT slots even though the
     // groups do not fit; the first keys a CTA sees (the hot head of a skewed distribution) aggregate in shared
     // memory, everything else falls through to the global table
-    const int hot_slots = [] { const char* e = getenv("BL_K5_HOT"); int v = e ? atoi(e) : 0; int c = 0; if (v > 0) { c = 16; while (c < v && c < 2048) c <<= 1; } return c; }();
+    const int hot_knob = knob_int("BL_K5_HOT", 0);
+    int hot_slots = 0; if (hot_knob > 0) { hot_slots = 16; while (hot_slots < hot_knob && hot_slots < 2048) hot_slots <<= 1; }
     if (!scap && hot_slots) scap = hot_slots;
     // tables that cannot stay L2-resident are filled in several passes over the batch: pass h only touches the
     // slot sub-range h of every plane (slot = top hash bits), so each pass works on an L2-sized slice
     int pass_bits = 0;
     if (!scap) {
-        const int mp = [] { const char* e = getenv("BL_K5_MULTIPASS"); return e ? atoi(e) : 1; }();
+        const int mp = knob_int("BL_K5_MULTIPASS", 1);
         const double tbl = (double)(cap + 2) * L.stride * 8, budget = 0.55 * (double)ctx().l2_bytes;
         while (mp && pass_bits < 3 && tbl / (double)(1 << pass_bits) > budget) pass_bits++;
         // every pass re-reads the batch: beyond 4 passes (or when even a quarter does not fit) the extra scans cost
         // more than the L2 misses they avoid
         if (pass_bits > 2) pass_bits = 0;
     }
-    GbTableDev Tp = T;
-    const bool use_hot = hot.rows > 0;
-#define GB_LAUNCH_ALL(E, C, KN)                                                      \
-    do { for (int h = 0; h < (1 << pass_bits); h++) { Tp.pass_bits = pass_bits; Tp.pass_id = h;                                              \
-             if (use_hot) launch_hot<E, C, KN>(Lb, Tp, B, hot, grid_hot); else launch_consume<E, C, KN>(Lb, Tp, B, grid); } } while (0)
-#define GB_DISPATCH(E, C)                                                            \
-    do { if (scap) { if (kn) launch_smem<E, C, true>(Lb, T, B, scap); else launch_smem<E, C, false>(Lb, T, B, scap); }                       \
-         else if (kn) GB_LAUNCH_ALL(E, C, true); else GB_LAUNCH_ALL(E, C, false); } while (0)
-    if (elem == 8) { if (canon == 1) GB_DISPATCH(8, 1); else GB_DISPATCH(8, 0); }
-    else { if (canon == 2) GB_DISPATCH(4, 2); else GB_DISPATCH(4, 0); }
-#undef GB_DISPATCH
-#undef GB_LAUNCH_ALL
+    with_key_form(key.dtype, [&](auto elem, auto canon) { with_bool(key.validity != nullptr, [&](auto kn) {
+        constexpr int E = decltype(elem)::value, C = decltype(canon)::value;
+        constexpr bool KN = decltype(kn)::value;
+        if (scap) { launch_smem<E, C, KN>(Lb, T, B, scap); return; }
+        GbTableDev Tp = T;
+        for (int h = 0; h < (1 << pass_bits); h++) {
+            Tp.pass_bits = pass_bits; Tp.pass_id = h;
+            if (hot.rows > 0) launch_hot<E, C, KN>(Lb, Tp, B, hot, grid_hot); else launch_consume<E, C, KN>(Lb, Tp, B, grid);
+        }
+    }); });
 }
 
 // does the batch have the shape k_gb_consume_lean takes?  (decides the table layout, so it is asked before alloc_table)
@@ -1462,13 +1279,11 @@ void GroupByState::consume_pipelined(const DevCol& key, const std::vector<const 
     PLB_REQUIRE(key.len <= 0xFFFFFFFEll, BL_ERR_UNSUPPORTED, "group_by: more than 2^32-2 rows (IdxSize = u32)");
     Context& c = ctx();
     const int64_t n = key.len;
-    const int es = dtype_size(key.dtype);
     auto slice = [&](const DevCol& col, int64_t lo, int64_t len) {
         DevCol s; s.dtype = col.dtype; s.len = len; s.null_count = 0;
         s.values = dev_borrow((const char*)col.v() + lo * dtype_size(col.dtype), (size_t)len * dtype_size(col.dtype));
         return s;
     };
-    (void)es;
     for (size_t ci = 0; ci < ready.size(); ci++) {
         const int64_t lo = (int64_t)ci * chunk_rows, len = std::min<int64_t>(chunk_rows, n - lo);
         PLB_CUDA(cudaStreamWaitEvent(c.stream, ready[ci], 0));
@@ -1580,7 +1395,7 @@ DevPtr GroupByState::export_partials(int n_partitions, int* row_words_out, int64
     const int row_words = L.n_words + 3;
     *row_words_out = row_words;
     if (!entries) { for (int p = 0; p <= n_partitions; p++) offsets_host[p] = 0; return dev_alloc(16); }
-    DevPtr counts = dev_alloc(8 * EXP_MAX_PARTS), cursor = dev_alloc(8 * EXP_MAX_PARTS), off = dev_alloc(8 * EXP_MAX_PARTS);
+    DevPtr counts = dev_alloc(8 * EXP_MAX_PARTS), cursor = dev_alloc(8 * EXP_MAX_PARTS);
     dev_memset(counts->p, 0, 8 * EXP_MAX_PARTS); dev_memset(cursor->p, 0, 8 * EXP_MAX_PARTS);
     PLB_LAUNCH("k6_export_count", k_gb_export_count, grid_for((int64_t)cap + 2, 256), 256, 0, T.entries, (int64_t)cap, T.es, n_partitions, as<unsigned long long>(counts));
     unsigned long long h[EXP_MAX_PARTS];
@@ -1589,13 +1404,14 @@ DevPtr GroupByState::export_partials(int n_partitions, int* row_words_out, int64
     unsigned long long ho[EXP_MAX_PARTS + 1]; ho[0] = 0;
     for (int p = 0; p < n_partitions; p++) ho[p + 1] = ho[p] + h[p];
     for (int p = 0; p <= n_partitions; p++) offsets_host[p] = (int64_t)ho[p];
-    PLB_CUDA(cudaMemcpyAsync(off->p, ho, 8 * n_partitions, cudaMemcpyHostToDevice, ctx().stream));
     const int64_t G = (int64_t)ho[n_partitions];
     DevPtr rows = dev_alloc((size_t)std::max<int64_t>(G, 1) * row_words * 8);
-    if (G > 0)
-        PLB_LAUNCH("k6_export_scatter", k_gb_export_scatter, grid_for((int64_t)cap + 2, 256), 256, 0, T.entries, (int64_t)cap, T.es, T.ws, T.pw, L.n_words, n_partitions,
-                   as<unsigned long long>(off), as<unsigned long long>(cursor), as<uint64_t>(rows));
-    PLB_CUDA(cudaStreamSynchronize(ctx().stream));   // ho[] is on this stack frame
+    PartDst D; memset(&D, 0, sizeof D);
+    for (int p = 0; p < n_partitions; p++) D.base[p] = as<uint64_t>(rows) + ho[p] * row_words;
+    if (G > 0)      // regions sized by the counts: no limit, no overflow flag
+        PLB_LAUNCH("k6_export_scatter", k_gb_export_scatter, grid_for((int64_t)cap + 2, 256), 256, 0, T.entries, (int64_t)cap, T.es, T.ws, T.pw, L.n_words, n_partitions, D,
+                   INT64_MAX, as<unsigned long long>(cursor), (int*)nullptr);
+    PLB_CUDA(cudaStreamSynchronize(ctx().stream));
     return rows;
 }
 
@@ -1605,12 +1421,15 @@ void GroupByState::export_partials_p2p(int n_ranks, int my_rank, void* const* wi
     *row_words_out = row_words;
     for (int p = 0; p < n_ranks; p++) sent_rows[p] = 0;
     if (!entries) return;
-    PeerWindows W; memset(&W, 0, sizeof W);
-    for (int p = 0; p < n_ranks; p++) { PLB_REQUIRE(windows[p] != nullptr, BL_ERR_INVALID, "export_partials_p2p: null window"); W.base[p] = reinterpret_cast<uint64_t*>(windows[p]); }
+    PartDst D; memset(&D, 0, sizeof D);      // partition p -> region my_rank of rank p's window
+    for (int p = 0; p < n_ranks; p++) {
+        PLB_REQUIRE(windows[p] != nullptr, BL_ERR_INVALID, "export_partials_p2p: null window");
+        D.base[p] = reinterpret_cast<uint64_t*>(windows[p]) + (int64_t)my_rank * rows_per_src * row_words;
+    }
     DevPtr cursor = dev_alloc(8 * EXP_MAX_PARTS), ovf = dev_alloc(4);
     dev_memset(cursor->p, 0, 8 * EXP_MAX_PARTS); dev_memset(ovf->p, 0, 4);
-    PLB_LAUNCH("k6_export_p2p", k_gb_export_p2p, grid_for((int64_t)cap + 2, 256), 256, 0, T.entries, (int64_t)cap, T.es, T.ws, T.pw, L.n_words, n_ranks, W,
-               rows_per_src * row_words, my_rank, rows_per_src, as<unsigned long long>(cursor), as<int>(ovf));
+    PLB_LAUNCH("k6_export_p2p", k_gb_export_scatter, grid_for((int64_t)cap + 2, 256), 256, 0, T.entries, (int64_t)cap, T.es, T.ws, T.pw, L.n_words, n_ranks, D,
+               rows_per_src, as<unsigned long long>(cursor), as<int>(ovf));
     unsigned long long h[EXP_MAX_PARTS];
     PLB_CUDA(cudaMemcpyAsync(h, cursor->p, 8 * n_ranks, cudaMemcpyDeviceToHost, ctx().stream));
     const int o = read_scalar(as<int>(ovf));      // also completes the kernel and its peer stores
@@ -1623,7 +1442,7 @@ void GroupByState::export_partials_p2p_async(int n_ranks, int my_rank, void* con
     PLB_REQUIRE(epoch > 0, BL_ERR_INVALID, "export_partials_p2p_async: epoch must be positive");
     const int row_words = L.n_words + 3;
     *row_words_out = row_words;
-    PeerWindows W; memset(&W, 0, sizeof W);
+    PartDst W; memset(&W, 0, sizeof W);
     for (int p = 0; p < n_ranks; p++) { PLB_REQUIRE(window_halves[p] != nullptr, BL_ERR_INVALID, "export_partials_p2p_async: null window"); W.base[p] = reinterpret_cast<uint64_t*>(window_halves[p]); }
     if (!entries) alloc_table(1024);          // nothing consumed: still publish zero counts so that no peer waits
     DevPtr ctl = dev_alloc(8 * EXP_MAX_PARTS + 8);

@@ -1,8 +1,30 @@
 // groupby.h — shared definitions + host-side state of the fused hash group_by (K5); see groupby.cu.
 #pragma once
+#include <cstdlib>
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace plb {
+
+// tuning knobs (environment variables): read on every call, so that they can change between calls
+inline int knob_int(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }
+inline double knob_double(const char* name, double dflt) { const char* e = getenv(name); return e ? atof(e) : dflt; }
+
+// ---- host dispatch onto kernel template arguments: f receives std::integral_constant arguments
+template <int V> using IntC = std::integral_constant<int, V>;
+// key form of a key dtype: f(element size 4 / 8, canonicalisation 0 raw bits / 1 f64 / 2 f32)
+template <class F> void with_key_form(int key_dtype, F&& f) {
+    if (dtype_size(key_dtype) == 8) { if (key_dtype == BL_FLOAT64) f(IntC<8>{}, IntC<1>{}); else f(IntC<8>{}, IntC<0>{}); }
+    else { if (key_dtype == BL_FLOAT32) f(IntC<4>{}, IntC<2>{}); else f(IntC<4>{}, IntC<0>{}); }
+}
+// f(the first V of Vs with n <= V; the last one otherwise)
+template <int V, int... Vs, class F> void with_at_least(int n, F&& f) {
+    if constexpr (sizeof...(Vs) == 0) f(IntC<V>{});
+    else if (n <= V) f(IntC<V>{});
+    else with_at_least<Vs...>(n, f);
+}
+template <class F> void with_bool(bool b, F&& f) { if (b) f(std::true_type{}); else f(std::false_type{}); }
 
 constexpr uint64_t GB_EMPTY = 0x8000000000000000ULL;   // i64::MIN / -0.0 bits (never a canonical float key)
 constexpr uint64_t GB_W1_INIT = 0xFFFFFFFF00000000ULL;  // first = u32::MAX, len = 0
@@ -100,6 +122,8 @@ struct GroupByState {
 
    private:
     void alloc_table(uint64_t new_cap);
+    int smem_table_cap() const;
+    bool bind_columns(const DevCol& key, const std::vector<const DevCol*>& values, int64_t row_base, int pw, int max_cols, GbBatch& B, GbLayout& Lb) const;
     void note_batch_shape(const DevCol& key, const std::vector<const DevCol*>& values);
     uint64_t choose_cap(const DevCol& key, int64_t n_total);
     void build_hot_list(const void* candidates, int n_cand, bool null_hot, bool empty_hot, double sample_rows);

@@ -46,6 +46,73 @@ __device__ __forceinline__ uint64_t raw_to_int(int dtype, uint64_t raw) {
     return dtype == BL_INT32 ? (uint64_t)(long long)(int)(uint32_t)raw : raw;   // sign-extend i32; u32 already zero-extended
 }
 
+// rows r0 and r0 + 1 of a column of ELEM-byte values: one 128-bit (8-byte types) or 64-bit (4-byte types) streaming load
+template <int ELEM> __device__ __forceinline__ void gb_load_pair(const void* col, int64_t r0, uint64_t& a, uint64_t& b) {
+    if (ELEM == 8) { const ulonglong2 t = ld_stream_u64x2(reinterpret_cast<const uint64_t*>(col) + r0); a = t.x; b = t.y; }
+    else { const uint2 t = ld_stream_u32x2(reinterpret_cast<const uint32_t*>(col) + r0); a = t.x; b = t.y; }
+}
+__device__ __forceinline__ void gb_load_pair_rt(const void* col, int elem, int64_t r0, uint64_t& a, uint64_t& b) {
+    if (elem == 8) gb_load_pair<8>(col, r0, a, b); else gb_load_pair<4>(col, r0, a, b);
+}
+
+// ---- global-memory accumulators: REDs, optionally with an L2 cache-policy hint (groupby.cu: make_policy_evict_last)
+__device__ __forceinline__ void red_add_u64(uint64_t* p, uint64_t v, uint64_t pol, bool hint) {
+    if (hint) asm volatile("red.global.add.L2::cache_hint.u64 [%0], %1, %2;" :: "l"(p), "l"(v), "l"(pol) : "memory");
+    else atomicAdd(reinterpret_cast<unsigned long long*>(p), (unsigned long long)v);
+}
+__device__ __forceinline__ void red_add_f64(uint64_t* p, double v, uint64_t pol, bool hint) {
+    if (hint) asm volatile("red.global.add.L2::cache_hint.f64 [%0], %1, %2;" :: "l"(p), "d"(v), "l"(pol) : "memory");
+    else atomicAdd(reinterpret_cast<double*>(p), v);
+}
+__device__ __forceinline__ void red_add_u32(uint32_t* p, uint32_t v, uint64_t pol, bool hint) {
+    if (hint) asm volatile("red.global.add.L2::cache_hint.u32 [%0], %1, %2;" :: "l"(p), "r"(v), "l"(pol) : "memory");
+    else atomicAdd(p, v);
+}
+// an integer 0 or a float +-0.0 is not added: the accumulator starts at 0 / +0.0 and never becomes -0.0, so the bits agree
+__device__ __forceinline__ void gb_apply(int op, uint64_t* addr, int dtype, uint64_t raw, bool valid, uint64_t pol = 0, bool hint = false) {
+    switch (op) {
+        case W_ADD_INT: { uint64_t v = raw_to_int(dtype, raw); if (valid && v) red_add_u64(addr, v, pol, hint); break; }
+        case W_ADD_F64: { double f = raw_to_f64(dtype, raw); if (valid && f != 0.0) red_add_f64(addr, f, pol, hint); break; }
+        case W_MIN_S64: if (valid) atomicMin(reinterpret_cast<long long*>(addr), (long long)raw_to_int(dtype, raw)); break;
+        case W_MAX_S64: if (valid) atomicMax(reinterpret_cast<long long*>(addr), (long long)raw_to_int(dtype, raw)); break;
+        case W_MIN_U64: if (valid) atomicMin(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)raw); break;
+        case W_MAX_U64: if (valid) atomicMax(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)raw); break;
+        case W_MIN_F64: { double f = raw_to_f64(dtype, raw); if (valid && f == f) atomicMin(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)f64_to_ordered(f)); break; }
+        case W_MAX_F64: { double f = raw_to_f64(dtype, raw); if (valid && f == f) atomicMax(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)f64_to_ordered(f)); break; }
+        default: if (!valid) atomicAdd(reinterpret_cast<unsigned long long*>(addr), 1ull); break;   // W_NULLCNT
+    }
+}
+// every accumulator word of one row: val(c) = the row's raw value in column c, word(w) = address of accumulator word w.
+// skip_pair: word L.pair_k travels in a bulk reduce instead.  MAXC >= L.n_cols: the row loops, column loop unrolled
+// (values in registers).  MAXC = 0: a plain loop for the odd tail row, value loaded once per column.  The two loops
+// are written so that the row-loop kernels get the same ptxas allocation as the hand-inlined code they replace: an
+// `#pragma unroll (expr)` form, or the value hoisted in the unrolled loop, moved registers and spills in some of them.
+template <int MAXC, class Val, class Word>
+__device__ __forceinline__ void gb_apply_words(const GbLayout& L, const GbBatch& B, int64_t row, Val val, Word word, uint64_t pol = 0, bool hint = false, bool skip_pair = false) {
+    if constexpr (MAXC > 0) {
+#pragma unroll
+        for (int c = 0; c < MAXC; c++) {
+            if (c < L.n_cols) {
+                const bool valid = B.cols[c].validity == nullptr || bit_get(B.cols[c].validity, row);
+                const int dt = B.cols[c].dtype;
+                for (int k = L.col_kbegin[c]; k < L.col_kbegin[c + 1]; k++) {
+                    if (skip_pair && k == L.pair_k) continue;
+                    gb_apply(L.wop[k], word(L.wslot[k]), dt, val(c), valid, pol, hint);
+                }
+            }
+        }
+    } else {
+        for (int c = 0; c < L.n_cols; c++) {
+            const bool valid = B.cols[c].validity == nullptr || bit_get(B.cols[c].validity, row);
+            const uint64_t raw = val(c);
+            for (int k = L.col_kbegin[c]; k < L.col_kbegin[c + 1]; k++) {
+                if (skip_pair && k == L.pair_k) continue;
+                gb_apply(L.wop[k], word(L.wslot[k]), B.cols[c].dtype, raw, valid, pol, hint);
+            }
+        }
+    }
+}
+
 
 // ---- shared-memory accumulators: 32-bit native ATOMS; 64-bit integer adds as two 32-bit adds with carry (exact,
 //      order-free); f64 add and 64-bit min/max are CAS loops (ATOMS.CAST.SPIN.64).

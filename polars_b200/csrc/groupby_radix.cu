@@ -48,15 +48,11 @@ struct GbRadixDev {
     int* status;
 };
 
+// gb_load_pair of rows r0, r0 + 1 with a bounds check against n (rows past the end read as 0)
 template <int KEY_ELEM> __device__ __forceinline__ void gbr_load_pair(const void* col, int64_t r0, int64_t n, uint64_t& a, uint64_t& b) {
     a = 0; b = 0;
-    if (KEY_ELEM == 8) {
-        if (r0 + 1 < n) { const ulonglong2 t = ld_stream_u64x2(reinterpret_cast<const uint64_t*>(col) + r0); a = t.x; b = t.y; }
-        else if (r0 < n) a = reinterpret_cast<const uint64_t*>(col)[r0];
-    } else {
-        if (r0 + 1 < n) { const uint2 t = ld_stream_u32x2(reinterpret_cast<const uint32_t*>(col) + r0); a = t.x; b = t.y; }
-        else if (r0 < n) a = reinterpret_cast<const uint32_t*>(col)[r0];
-    }
+    if (r0 + 1 < n) gb_load_pair<KEY_ELEM>(col, r0, a, b);
+    else if (r0 < n) a = KEY_ELEM == 8 ? reinterpret_cast<const uint64_t*>(col)[r0] : reinterpret_cast<const uint32_t*>(col)[r0];
 }
 __device__ __forceinline__ void gbr_load_pair_rt(const void* col, int elem, int64_t r0, int64_t n, uint64_t& a, uint64_t& b) {
     if (elem == 8) gbr_load_pair<8>(col, r0, n, a, b); else gbr_load_pair<4>(col, r0, n, a, b);
@@ -113,6 +109,9 @@ __global__ void __launch_bounds__(1024) k_gbr_offsets(const unsigned* __restrict
 }
 
 // ---------------------------------------------------------------------------- pass 1: tile sort + TMA bulk stores
+// the GB_EMPTY key is the pad marker of the record streams: its (rare) rows aggregate straight into sp = [len, words...].
+// Not gb_apply: inlined into the scatters, gb_apply changed ptxas's register allocation of every k_gbr_scatter /
+// k_gbr_scatter_wc instantiation (k_gbr_scatter_wc<3, 8, 0>: a 16-byte frame without spills became 64 bytes with spills).
 __device__ __forceinline__ void gbr_apply_special(const GbLayout& L, const GbBatch& Bt, uint64_t* sp, const uint64_t* raw) {
     atomicAdd(reinterpret_cast<unsigned long long*>(sp), 1ull);
     for (int c = 0; c < L.n_cols; c++)
@@ -133,9 +132,10 @@ __device__ __forceinline__ void gbr_apply_special(const GbLayout& L, const GbBat
         }
 }
 
-template <int ROWW, int KEY_ELEM, int KEY_CANON, bool BULK, int RPT>
+constexpr int GBR_RPT = 4;      // rows per thread: 2048-row tiles (8 rows per thread, 4096-row tiles at 1 CTA / SM, was slower)
+template <int ROWW, int KEY_ELEM, int KEY_CANON, bool BULK>
 __global__ void __launch_bounds__(GBR_THREADS) k_gbr_scatter(const __grid_constant__ GbLayout L, const __grid_constant__ GbBatch Bt, const __grid_constant__ GbRadixDev R) {
-    constexpr int T = GBR_THREADS * RPT, THREADS = GBR_THREADS, NC = ROWW - 1;
+    constexpr int RPT = GBR_RPT, T = GBR_THREADS * RPT, THREADS = GBR_THREADS, NC = ROWW - 1;
     const int logB = R.logB, B = 1 << logB;
     extern __shared__ __align__(16) uint64_t gbr_smem[];
     uint64_t* stage = gbr_smem;                                        // (T + (BULK ? B : 0)) records
@@ -358,9 +358,10 @@ __global__ void __launch_bounds__(GBR_WC_THREADS, 2) k_gbr_scatter_wc(const __gr
 // ---------------------------------------------------------------------------- pass 2: TMA ring -> shared-memory table -> dense output
 struct GbDenseDev { uint64_t* keys; uint32_t* first; uint32_t* len; uint64_t* words; int64_t Gb; unsigned long long* cursor; };
 
-template <int ROWW, int K, int NST>
+constexpr int GBR_NST = 2;      // ring stages
+template <int ROWW>
 __global__ void __launch_bounds__(1024) k_gbr_agg(const __grid_constant__ GbLayout L, const __grid_constant__ GbBatch Bt, const __grid_constant__ GbRadixDev R, const __grid_constant__ GbDenseDev D, unsigned S) {
-    constexpr int CR = GBR_NCW * 32 * K, NC = ROWW - 1;
+    constexpr int NST = GBR_NST, CR = GBR_NCT, NC = ROWW - 1;      // one record per consumer thread and stage
     extern __shared__ __align__(128) uint64_t gbr_smem2[];
     uint64_t* ring = gbr_smem2;                                       // NST x CR records
     uint64_t* tkey = ring + (size_t)NST * CR * ROWW;                  // S keys
@@ -403,42 +404,35 @@ __global__ void __launch_bounds__(1024) k_gbr_agg(const __grid_constant__ GbLayo
             while (!mbar_try_wait(&full[st], par)) {}
             const uint64_t* buf = ring + (size_t)st * CR * ROWW;
             const int crow = (int)min((int64_t)CR, rows - (int64_t)c * CR);
-            uint64_t rec[K][ROWW];
+            uint64_t rec[ROWW];
+            rec[0] = GB_EMPTY;
+            if (tid < crow) {
 #pragma unroll
-            for (int u = 0; u < K; u++) {
-                const int r = (warp * K + u) * 32 + lane;
-                rec[u][0] = GB_EMPTY;
-                if (r < crow) {
-#pragma unroll
-                    for (int w = 0; w < ROWW; w++) rec[u][w] = buf[r * ROWW + w];
-                }
+                for (int w = 0; w < ROWW; w++) rec[w] = buf[tid * ROWW + w];
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty[st]);
-#pragma unroll
-            for (int u = 0; u < K; u++) {
-                const uint64_t key = rec[u][0];
-                if (key == GB_EMPTY) continue;              // pad record
-                unsigned slot = __umulhi((unsigned)((table_hash(key) << R.logB) >> 32), S);
-                bool found = false;
-                for (unsigned probes = 0; probes < 128u; probes++) {
-                    const uint64_t cur = *reinterpret_cast<volatile uint64_t*>(tkey + slot);
-                    if (cur == key) { found = true; break; }
-                    if (cur == GB_EMPTY) {
-                        if (*reinterpret_cast<volatile unsigned*>(&s_used) >= max_used) break;
-                        const unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(tkey + slot), (unsigned long long)GB_EMPTY, (unsigned long long)key);
-                        if (old == GB_EMPTY) { atomicAdd(&s_used, 1u); found = true; break; }
-                        if (old == key) { found = true; break; }
-                    }
-                    if (++slot == S) slot = 0;
+            const uint64_t key = rec[0];
+            if (key == GB_EMPTY) continue;              // pad record
+            unsigned slot = __umulhi((unsigned)((table_hash(key) << R.logB) >> 32), S);
+            bool found = false;
+            for (unsigned probes = 0; probes < 128u; probes++) {
+                const uint64_t cur = *reinterpret_cast<volatile uint64_t*>(tkey + slot);
+                if (cur == key) { found = true; break; }
+                if (cur == GB_EMPTY) {
+                    if (*reinterpret_cast<volatile unsigned*>(&s_used) >= max_used) break;
+                    const unsigned long long old = atomicCAS(reinterpret_cast<unsigned long long*>(tkey + slot), (unsigned long long)GB_EMPTY, (unsigned long long)key);
+                    if (old == GB_EMPTY) { atomicAdd(&s_used, 1u); found = true; break; }
+                    if (old == key) { found = true; break; }
                 }
-                if (!found) { *R.status = 1; continue; }    // more groups in this bucket than its table holds: the caller falls back
-                if (L.need_len) atomicAdd(tlen + slot, 1u);
+                if (++slot == S) slot = 0;
+            }
+            if (!found) { *R.status = 1; continue; }    // more groups in this bucket than its table holds: the caller falls back
+            if (L.need_len) atomicAdd(tlen + slot, 1u);
 #pragma unroll
-                for (int cix = 0; cix < NC; cix++) {
-                    const int dt = Bt.cols[cix].dtype;
-                    for (int kk = L.col_kbegin[cix]; kk < L.col_kbegin[cix + 1]; kk++) gb_apply_smem<false>(L.wop[kk], tacc + (size_t)L.wslot[kk] * S + slot, dt, rec[u][1 + cix], true);
-                }
+            for (int cix = 0; cix < NC; cix++) {
+                const int dt = Bt.cols[cix].dtype;
+                for (int kk = L.col_kbegin[cix]; kk < L.col_kbegin[cix + 1]; kk++) gb_apply_smem<false>(L.wop[kk], tacc + (size_t)L.wslot[kk] * S + slot, dt, rec[1 + cix], true);
             }
         }
         named_bar_sync(1, GBR_NCT);
@@ -476,94 +470,57 @@ __global__ void k_gbr_append_special(const uint64_t* __restrict__ special, int n
 // =============================================================================================
 // Host side
 // =============================================================================================
-constexpr int GBR_RPT_BULK = 4, GBR_RPT_PLAIN = 4;      // 8 rows per thread (4096-row tiles, 1 CTA / SM) was slower
-static int64_t gbr_tile_rows(bool bulk) { return (int64_t)GBR_THREADS * (bulk ? GBR_RPT_BULK : GBR_RPT_PLAIN); }
 static size_t gbr_wc_smem(int B, int roww) { return (size_t)B * (GBR_WC_F * roww * 8 + 4); }
 // write-combining scatter: grid = the CTAs that fit at once (persistent; k_gbr_offsets pads for each of them)
 template <int ROWW, int KEY_ELEM, int KEY_CANON>
-static void scatter_wc_grid(int B, int& grid) {
+static int scatter_wc_grid(int B) {
     auto kfn = k_gbr_scatter_wc<ROWW, KEY_ELEM, KEY_CANON>;
     const size_t smem = gbr_wc_smem(B, ROWW);
     PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     PLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kfn, GBR_WC_THREADS, smem));
-    grid = ctx().sm_count * std::max(occ, 1);
-}
-template <int ROWW, int KEY_ELEM, int KEY_CANON>
-static void launch_scatter_wc(const GbLayout& L, const GbBatch& Bt, const GbRadixDev& R, int grid) {
-    PLB_LAUNCH("k5r_scatter", (k_gbr_scatter_wc<ROWW, KEY_ELEM, KEY_CANON>), grid, GBR_WC_THREADS, gbr_wc_smem(1 << R.logB, ROWW), L, Bt, R);
+    return ctx().sm_count * std::max(occ, 1);
 }
 template <int ROWW, int KEY_ELEM, int KEY_CANON>
 static void launch_scatter(const GbLayout& L, const GbBatch& Bt, const GbRadixDev& R, bool bulk) {
     const int B = 1 << R.logB;
-    const size_t tile = (size_t)gbr_tile_rows(bulk);
+    const size_t tile = (size_t)GBR_THREADS * GBR_RPT;
     const size_t smem = (tile + (bulk ? B : 0)) * ROWW * 8 + (size_t)3 * B * 4 + (bulk ? 0 : tile * 2);
+    auto kfn = bulk ? k_gbr_scatter<ROWW, KEY_ELEM, KEY_CANON, true> : k_gbr_scatter<ROWW, KEY_ELEM, KEY_CANON, false>;
+    PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
-    if (bulk) {
-        auto kfn = k_gbr_scatter<ROWW, KEY_ELEM, KEY_CANON, true, GBR_RPT_BULK>;
-        PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        PLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kfn, GBR_THREADS, smem));
-        PLB_LAUNCH("k5r_scatter", kfn, ctx().sm_count * std::max(occ, 1), GBR_THREADS, smem, L, Bt, R);
-    } else {
-        auto kfn = k_gbr_scatter<ROWW, KEY_ELEM, KEY_CANON, false, GBR_RPT_PLAIN>;
-        PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        PLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kfn, GBR_THREADS, smem));
-        PLB_LAUNCH("k5r_scatter", kfn, ctx().sm_count * std::max(occ, 1), GBR_THREADS, smem, L, Bt, R);
-    }
+    PLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kfn, GBR_THREADS, smem));
+    PLB_LAUNCH("k5r_scatter", kfn, ctx().sm_count * std::max(occ, 1), GBR_THREADS, smem, L, Bt, R);
 }
 template <int ROWW>
-static void launch_agg(const GbLayout& L, const GbBatch& Bt, const GbRadixDev& R, const GbDenseDev& D, unsigned S, int stages) {
-    const size_t table = (size_t)S * (8 + 4 + 8 * L.n_words);
-    const int B = 1 << R.logB;
-    auto go = [&](auto kfn, int k, int nst) {
-        const size_t smem = (size_t)nst * GBR_NCW * 32 * k * ROWW * 8 + table + 16;
-        PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int occ = 0;
-        PLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kfn, 1024, smem));
-        PLB_LAUNCH("k5r_aggregate", kfn, std::min(B, ctx().sm_count * std::max(occ, 1)), 1024, smem, L, Bt, R, D, S);
-    };
-    if (stages >= 4) go(k_gbr_agg<ROWW, 1, 4>, 1, 4); else go(k_gbr_agg<ROWW, 1, 2>, 1, 2);
+static void launch_agg(const GbLayout& L, const GbBatch& Bt, const GbRadixDev& R, const GbDenseDev& D, unsigned S) {
+    auto kfn = k_gbr_agg<ROWW>;
+    const size_t smem = (size_t)GBR_NST * GBR_NCT * ROWW * 8 + (size_t)S * (8 + 4 + 8 * L.n_words) + 16;      // ring + table
+    PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int occ = 0;
+    PLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kfn, 1024, smem));
+    PLB_LAUNCH("k5r_aggregate", kfn, std::min(1 << R.logB, ctx().sm_count * std::max(occ, 1)), 1024, smem, L, Bt, R, D, S);
 }
 
 // Returns false when the plan does not apply (or gave up): nothing is left behind and the caller runs the L2 plan.
 bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevCol*>& values, uint64_t planned_cap) {
-    const int mode = [] { const char* e = getenv("BL_K5_RADIX"); return e ? atoi(e) : 1; }();      // 0 never, 1 when the table would leave L2, 2 whenever eligible (read per call)
+    const int mode = knob_int("BL_K5_RADIX", 1);      // 0 never, 1 when the table would leave L2, 2 whenever eligible
     if (mode == 0 || L.need_first || key.validity != nullptr || hot.rows > 0 || key.len < (1 << 20)) return false;
-    // column binding (same rule as launch_batch: aggregations over one buffer share a record word)
-    GbBatch Bt; memset(&Bt, 0, sizeof Bt);
-    Bt.keys = key.v(); Bt.n = key.len; Bt.key_dtype = key.dtype;
-    std::vector<const void*> col_ptr; std::vector<int> col_of_agg(plans.size(), -1);
+    // records carry 4- or 8-byte values without validity, at most 4 value columns
     for (size_t i = 0; i < plans.size(); i++) {
         if (plans[i].kind == BL_AGG_LEN) continue;
         const DevCol* v = values[i];
         if (v == nullptr || v->len != key.len || v->dtype != plans[i].in_dtype || v->validity != nullptr) return false;
         if (dtype_size(v->dtype) != 4 && dtype_size(v->dtype) != 8) return false;
-        int c = -1;
-        for (size_t j = 0; j < col_ptr.size(); j++) if (col_ptr[j] == v->v()) c = (int)j;
-        if (c < 0) {
-            if (col_ptr.size() >= 4) return false;
-            c = (int)col_ptr.size(); col_ptr.push_back(v->v());
-            Bt.cols[c].values = v->v(); Bt.cols[c].validity = nullptr; Bt.cols[c].dtype = v->dtype; Bt.cols[c].elem = dtype_size(v->dtype);
-        }
-        col_of_agg[i] = c;
     }
-    GbLayout Lb = L;
-    Lb.n_cols = (int)col_ptr.size();
-    int kk = 0;
-    for (int c = 0; c < Lb.n_cols; c++) {
-        Lb.col_kbegin[c] = kk;
-        for (size_t i = 0; i < plans.size(); i++) {
-            if (col_of_agg[i] != c) continue;
-            if (plans[i].main >= 0) { Lb.wslot[kk] = plans[i].main; Lb.wop[kk] = L.slot_op[plans[i].main]; kk++; }
-        }
-    }
-    for (int c = Lb.n_cols; c <= GB_MAX_COLS; c++) Lb.col_kbegin[c] = kk;
+    GbBatch Bt; GbLayout Lb;
+    if (!bind_columns(key, values, 0, 0, 4, Bt, Lb)) return false;
     const int roww = 1 + Lb.n_cols;
     const int64_t n = key.len;
     // shared-memory table per bucket: what is left of ~110 KB (2 CTAs / SM) after a
     // 2-stage ring; when even 8192 buckets of that size cannot take the estimated groups, one CTA / SM with a ~200 KB table
     const size_t entry = 8 + 4 + 8 * (size_t)L.n_words;
-    const size_t ring2 = (size_t)2 * GBR_NCW * 32 * roww * 8;
+    const size_t ring2 = (size_t)GBR_NST * GBR_NCT * roww * 8;
     unsigned S = 0; int logB = 6;
     for (const size_t total_kb : {(size_t)110, (size_t)222}) {
         if (total_kb * 1024 < ring2 + 1024 + 512 * entry) continue;
@@ -588,16 +545,11 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
     int smem_optin = 0;
     PLB_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx().device));
     const bool wc = !bulk && gbr_wc_smem(B, roww) <= (size_t)smem_optin;
-    const int64_t ntiles = (n + gbr_tile_rows(bulk) - 1) / gbr_tile_rows(bulk);
-    const int elem = dtype_size(key.dtype);
-    const int canon = key.dtype == BL_FLOAT64 ? 1 : (key.dtype == BL_FLOAT32 ? 2 : 0);
-#define GBR_KEYS(CALL) do { if (elem == 8) { if (canon == 1) { CALL(8, 1); } else { CALL(8, 0); } } else { if (canon == 2) { CALL(4, 2); } else { CALL(4, 0); } } } while (0)
-#define GBR_ROWW(FN, E, CN, ...) do { switch (roww) { case 1: FN<1, E, CN>(__VA_ARGS__); break; case 2: FN<2, E, CN>(__VA_ARGS__); break; case 3: FN<3, E, CN>(__VA_ARGS__); break; \
-                                                      case 4: FN<4, E, CN>(__VA_ARGS__); break; default: FN<5, E, CN>(__VA_ARGS__); break; } } while (0)
+    const int64_t ntiles = (n + GBR_THREADS * GBR_RPT - 1) / (GBR_THREADS * GBR_RPT);
+    // f(KEY_ELEM, KEY_CANON, ROWW) of the scatter kernels for this batch
+    auto with_scatter_form = [&](auto f) { with_key_form(key.dtype, [&](auto e, auto c) { with_at_least<1, 2, 3, 4, 5>(roww, [&](auto w) { f(e, c, w); }); }); };
     int wc_grid = 0;
-#define WCGRID(E, CN) GBR_ROWW(scatter_wc_grid, E, CN, B, wc_grid)
-    if (wc) GBR_KEYS(WCGRID);
-#undef WCGRID
+    if (wc) with_scatter_form([&](auto e, auto c, auto w) { wc_grid = scatter_wc_grid<decltype(w)::value, decltype(e)::value, decltype(c)::value>(B); });
     const int64_t pad_rows = bulk ? std::min<int64_t>(n, (int64_t)B * ntiles) : wc ? std::min<int64_t>(n, (int64_t)B * wc_grid) * (GBR_WC_F - 1) : 0;
     const int64_t rec_rows = n + pad_rows + (wc ? GBR_WC_F : 2) * (int64_t)B + 16;
     DevPtr recs, ctl;
@@ -619,17 +571,16 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
         PLB_CUDA(cudaStreamSynchronize(ctx().stream));      // h lives on this frame
     }
     dev_memset(status->p, 0, 4);
-    const int hgrid = ctx().sm_count * 4;
-#define HIST(E, CN) PLB_LAUNCH("k5r_histogram", (k_gbr_hist<E, CN>), hgrid, 512, (size_t)B * 4, key.v(), n, logB, R.counts)
-    GBR_KEYS(HIST);
-#undef HIST
+    with_key_form(key.dtype, [&](auto e, auto c) {
+        PLB_LAUNCH("k5r_histogram", (k_gbr_hist<decltype(e)::value, decltype(c)::value>), ctx().sm_count * 4, 512, (size_t)B * 4, key.v(), n, logB, R.counts);
+    });
     if (wc) PLB_LAUNCH("k5r_offsets", k_gbr_offsets, 1, 1024, 0, R.counts, B, (unsigned long long)wc_grid, (unsigned)(GBR_WC_F - 1), (unsigned)GBR_WC_F, const_cast<unsigned long long*>(R.off), R.cursor);
     else PLB_LAUNCH("k5r_offsets", k_gbr_offsets, 1, 1024, 0, R.counts, B, (unsigned long long)ntiles, bulk ? 1u : 0u, 2u, const_cast<unsigned long long*>(R.off), R.cursor);
-#define SCAT(E, CN) do { if (wc) GBR_ROWW(launch_scatter_wc, E, CN, Lb, Bt, R, wc_grid); else GBR_ROWW(launch_scatter, E, CN, Lb, Bt, R, bulk); } while (0)
-    GBR_KEYS(SCAT);
-#undef SCAT
-#undef GBR_ROWW
-#undef GBR_KEYS
+    with_scatter_form([&](auto e, auto c, auto w) {
+        constexpr int E = decltype(e)::value, C = decltype(c)::value, ROWW = decltype(w)::value;
+        if (wc) PLB_LAUNCH("k5r_scatter", (k_gbr_scatter_wc<ROWW, E, C>), wc_grid, GBR_WC_THREADS, gbr_wc_smem(B, ROWW), Lb, Bt, R);
+        else launch_scatter<ROWW, E, C>(Lb, Bt, R, bulk);
+    });
     // dense output, sized by a generous bound on the group count (overflow -> status -> fall back)
     const int64_t Gb = std::max<int64_t>(1024, std::min<int64_t>(n + 1, 3 * est_groups + (1 << 16)));
     dense.keys = dev_alloc((size_t)Gb * 8); dense.first = dev_alloc((size_t)Gb * 4); dense.len = dev_alloc((size_t)Gb * 4);
@@ -637,10 +588,7 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
     const long long ctl_init[2] = {0, -1};
     PLB_CUDA(cudaMemcpyAsync(dense.ctl->p, ctl_init, 16, cudaMemcpyHostToDevice, ctx().stream));
     GbDenseDev D{as<uint64_t>(dense.keys), as<uint32_t>(dense.first), as<uint32_t>(dense.len), as<uint64_t>(dense.words), Gb, as<unsigned long long>(dense.ctl)};
-    switch (roww) {
-        case 1: launch_agg<1>(Lb, Bt, R, D, S, 2); break; case 2: launch_agg<2>(Lb, Bt, R, D, S, 2); break; case 3: launch_agg<3>(Lb, Bt, R, D, S, 2); break;
-        case 4: launch_agg<4>(Lb, Bt, R, D, S, 2); break; default: launch_agg<5>(Lb, Bt, R, D, S, 2); break;
-    }
+    with_at_least<1, 2, 3, 4, 5>(roww, [&](auto w) { launch_agg<decltype(w)::value>(Lb, Bt, R, D, S); });
     PLB_LAUNCH("k5r_special", k_gbr_append_special, 1, 32, 0, R.special, L.n_words, D, as<int>(status));
     const int st = read_scalar(as<int>(status));      // also orders ctl_init / recs lifetimes
     if (getenv("BL_K5_DEBUG")) fprintf(stderr, "[k5r] rows=%lld est_groups=%lld buckets=%d slots=%u bulk=%d store=%s status=%d\n", (long long)n, (long long)est_groups, B, S, (int)bulk,

@@ -376,7 +376,8 @@ def test_deterministic_plan(plb, monkeypatch):
 # ------------------------------------------------------------------ streaming, rehash, export / merge, P2P window
 def test_streaming_rehash_merge(plb):
     """GroupBy.consume in three batches whose new keys force the table to grow (k5_rehash), export_partials(2) +
-    merge_partials (k5_merge_partials) into a fresh state, and the P2P window merge into our own window."""
+    merge_partials (k5_merge_partials) into a fresh state, the synchronous P2P export (export_partials_p2p) merged back
+    with merge_partials, and the P2P window merge into our own window."""
     rng = np.random.default_rng(2024)
     case = ref.Case(rng, "int64", big=BIG, singletons=20_000, groups=100_000, rest=600_000, big_key=np.iinfo(np.int64).min)
     # batches: the first holds a few hundred keys, so the table is sized small; the next two bring ~100 000 new keys
@@ -416,6 +417,19 @@ def test_streaming_rehash_merge(plb):
     check(res, "export + merge")
     groups = int(offs[-1])
     rows_per_src = groups + 1024
+    # synchronous P2P export as rank 1 of 2: partition p's rows land in region 1 of window p; merge_partials reads both
+    wins = [plb.Window(2 * rows_per_src * rw * 8) for _ in range(2)]
+    try:
+        rw_p2p, sent = t.export_partials_p2p([w.ptr for w in wins], 1, rows_per_src)
+        assert rw_p2p == rw and sent.tolist() == np.diff(offs).tolist(), (rw_p2p, rw, sent, offs)
+        q = plb.GroupBy(np.int64, spec, nullable=nn)
+        for w, c in zip(wins, sent):
+            q.merge_partials(w.ptr + rows_per_src * rw * 8, int(c))
+        check(q.finish(), "p2p export + merge")
+        del q
+    finally:
+        for w in wins:
+            w.destroy()
     win = plb.Window(1024 + rows_per_src * rw * 8)
     try:
         t.export_partials_p2p_async([win.ptr], 0, rows_per_src, 1)
