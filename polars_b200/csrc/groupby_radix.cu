@@ -15,10 +15,10 @@
 //                           k_gbr_scatter writes the sorted tile with coalesced 8-byte stores (no padding).
 //   pass 2  k_gbr_agg       one CTA per bucket: the bucket's record stream is staged into shared memory by
 //                           cp.async.bulk (TMA) global->shared copies on an mbarrier ring (a producer warp issues,
-//                           31 consumer warps each release their slice of a stage on an `empty` mbarrier as soon as it
-//                           sits in registers); rows aggregate into a shared-memory open-addressing table; a bucket's
-//                           groups are final, so they leave compacted straight into the dense output arrays — the
-//                           global table, its initialisation and its extraction disappear.
+//                           31 consumer warps each release their slice of a stage on an `empty` mbarrier, behind a
+//                           proxy fence, as soon as it sits in registers); rows aggregate into a shared-memory
+//                           open-addressing table; a bucket's groups are final, so they leave compacted straight into
+//                           the dense output arrays — the global table, its initialisation and its extraction disappear.
 // While the L2 plan's table stays in L2 this plan loses to it (64-bit shared-memory atomics on random slots cost several
 // SM cycles per row), so it is only taken when the L2 plan's table would exceed the L2 budget.
 // Restrictions (anything else stays on the L2 plan): no validity bitmaps, no first-row tracking, <= 4 value columns,
@@ -410,6 +410,11 @@ __global__ void __launch_bounds__(1024) k_gbr_agg(const __grid_constant__ GbLayo
 #pragma unroll
                 for (int w = 0; w < ROWW; w++) rec[w] = buf[tid * ROWW + w];
             }
+            // the release below lets the producer's next TMA write overwrite this stage.  The warp signals before it uses
+            // the record, so nothing else waits for these loads: without the proxy fence, a copy issued on lane 0's arrival
+            // could land before another lane's load had read the stage (that lane then aggregated a record of the
+            // bucket's next chunk but one in place of its own)
+            fence_async_smem();
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty[st]);
             const uint64_t key = rec[0];
@@ -471,6 +476,11 @@ __global__ void k_gbr_append_special(const uint64_t* __restrict__ special, int n
 // Host side
 // =============================================================================================
 static size_t gbr_wc_smem(int B, int roww) { return (size_t)B * (GBR_WC_F * roww * 8 + 4); }
+// k_gbr_scatter: the staged tile (+ one pad record per bucket for the runs), hist / start / gpos, the bucket of every slot (coalesced)
+static size_t gbr_scatter_smem(int B, int roww, bool bulk) {
+    const size_t tile = (size_t)GBR_THREADS * GBR_RPT;
+    return (tile + (bulk ? B : 0)) * roww * 8 + (size_t)3 * B * 4 + (bulk ? 0 : tile * 2);
+}
 // write-combining scatter: grid = the CTAs that fit at once (persistent; k_gbr_offsets pads for each of them)
 template <int ROWW, int KEY_ELEM, int KEY_CANON>
 static int scatter_wc_grid(int B) {
@@ -483,9 +493,7 @@ static int scatter_wc_grid(int B) {
 }
 template <int ROWW, int KEY_ELEM, int KEY_CANON>
 static void launch_scatter(const GbLayout& L, const GbBatch& Bt, const GbRadixDev& R, bool bulk) {
-    const int B = 1 << R.logB;
-    const size_t tile = (size_t)GBR_THREADS * GBR_RPT;
-    const size_t smem = (tile + (bulk ? B : 0)) * ROWW * 8 + (size_t)3 * B * 4 + (bulk ? 0 : tile * 2);
+    const size_t smem = gbr_scatter_smem(1 << R.logB, ROWW, bulk);
     auto kfn = bulk ? k_gbr_scatter<ROWW, KEY_ELEM, KEY_CANON, true> : k_gbr_scatter<ROWW, KEY_ELEM, KEY_CANON, false>;
     PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
@@ -539,12 +547,17 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
         if ((double)planned_cap * L.stride * 8 <= 2.0 * l2_budget) return false;
     }
     const int B = 1 << logB;
-    const bool bulk = logB <= 9;
-    // many buckets: write-combining buffers when a chunk buffer per bucket fits one CTA's shared memory, else the
-    // tile is written with coalesced stores
+    // store path of the scatter: TMA runs up to 512 buckets; past that write-combining buffers when a chunk buffer per
+    // bucket fits one CTA's shared memory, else the tile is written with coalesced stores.  BL_K5R_STORE (1 coalesced,
+    // 2 write-combining, 3 runs) picks a path instead wherever its shared memory fits.
     int smem_optin = 0;
     PLB_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx().device));
-    const bool wc = !bulk && gbr_wc_smem(B, roww) <= (size_t)smem_optin;
+    const bool wc_fits = gbr_wc_smem(B, roww) <= (size_t)smem_optin;
+    const int store = knob_int("BL_K5R_STORE", 0);
+    bool bulk = logB <= 9, wc = !bulk && wc_fits;
+    if (store == 1 && gbr_scatter_smem(B, roww, false) <= (size_t)smem_optin) bulk = wc = false;
+    else if (store == 2 && wc_fits) { bulk = false; wc = true; }
+    else if (store == 3 && gbr_scatter_smem(B, roww, true) <= (size_t)smem_optin) { bulk = true; wc = false; }
     const int64_t ntiles = (n + GBR_THREADS * GBR_RPT - 1) / (GBR_THREADS * GBR_RPT);
     // f(KEY_ELEM, KEY_CANON, ROWW) of the scatter kernels for this batch
     auto with_scatter_form = [&](auto f) { with_key_form(key.dtype, [&](auto e, auto c) { with_at_least<1, 2, 3, 4, 5>(roww, [&](auto w) { f(e, c, w); }); }); };

@@ -9,7 +9,7 @@ CTA's shared memory holds (B * 4 records of ROWW words) the plan keeps the coale
 
 Record widths 1 to 5 words (key + up to 4 value columns) with 4- and 8-byte value columns, 4- and 8-byte keys, and the
 GB_EMPTY key (i64::MIN / u64 2^63: the pad marker of the record streams) on a group of 2^20 rows.  4-byte keys cannot
-carry that bit pattern; their cases have no group of 2^20 rows.  Row counts are multiples of n_loop(sm_count) from
+carry that bit pattern; their group of 2^20 rows is on an ordinary key.  Row counts are multiples of n_loop(sm_count) from
 test_gpu_groupby_plans.py with a ragged tail, so every CTA of the persistent grid ends with partial chunks.  Float keys are not covered here: group_by_agg tracks first rows for them, which keeps them on the
 L2 plan.  Integer aggregates and counts match bit for bit; float sums use exact-summable values.
 """
@@ -56,9 +56,8 @@ def test_radix_many_buckets(plb, sm, monkeypatch, capfd, name):
     rng = np.random.default_rng(len(name) * 7 + buckets)
     n = mult * n_loop(sm)
     singletons = 10_000
-    big = BIG if EMPTY_KEY[key_dt] is not None else 0
-    case = ref.Case(rng, key_dt, big=big, singletons=singletons, groups=groups,
-                    rest=n - big - singletons - sum(ref.SPECIAL_ROWS.values()), big_key=EMPTY_KEY[key_dt])
+    case = ref.Case(rng, key_dt, big=BIG, singletons=singletons, groups=groups,
+                    rest=n - BIG - singletons - sum(ref.SPECIAL_ROWS.values()), big_key=EMPTY_KEY[key_dt])
     cols = value_cols(case, rng, dts, False, exact=True)
     aggs = [("sum", c[1]) for c in cols]
     if minmax:

@@ -25,6 +25,7 @@ import pytest
 
 import join_keys as jk
 import oracle
+from radix_ref import key_with_hash
 
 pytestmark = pytest.mark.gpu
 
@@ -33,9 +34,6 @@ HOWS = ("inner", "left", "semi", "anti", "full")
 INNER_ORDERS = ("none", "left", "left_right", "right")
 LEFT_ORDERS = ("none", "left", "right", "right_left")
 BUILD_LABEL = {"dense": "k7_dense_build", "wide": "k7_join_build", "compact": "k7_jc_build"}
-M64 = (1 << 64) - 1
-_HASH_MUL = 0x9E3779B97F4A7C15                       # table_hash (dev_utils.cuh): (k ^ (k >> 31)) * _HASH_MUL
-_HASH_INV = pow(_HASH_MUL, -1, 1 << 64)
 
 
 @pytest.fixture(scope="module")
@@ -56,18 +54,6 @@ def n_build(sm):
 
 def n_probe(sm):
     return 36864 * sm + 1001
-
-
-def table_hash(k: int) -> int:
-    return ((k ^ (k >> 31)) * _HASH_MUL) & M64
-
-
-def key_with_hash(h: int) -> int:
-    """The 64-bit key whose table_hash is h (both steps of the hash are invertible)."""
-    x = (h * _HASH_INV) & M64
-    k = x ^ (x >> 31) ^ (x >> 62)
-    assert table_hash(k) == h
-    return k
 
 
 def wide_tail_keys(rng, n_rows: int, fill: float, count: int) -> list:
