@@ -458,9 +458,10 @@ __global__ void k_gb_init(uint64_t* entries, int64_t n_entries, int stride, int 
 // cardinality sample: insert m strided keys into a scratch key table with per-slot multiplicities.
 // stats[0] = distinct keys, stats[3] = sampled rows whose successor row carries the same key
 // (collision rate of neighbouring rows: skew / sortedness); stats[1], stats[2] are filled by
-// k_gb_estimate_stats (keys seen exactly once / exactly twice in the sample).
+// k_gb_estimate_stats (keys seen exactly once / exactly twice in the sample; pairs = sum of c (c - 1) over the sampled
+// multiplicities c, 64-bit: one key on all 65,536 sampled rows gives 4.3e9).
 constexpr int GB_CAND_MAX = 1024;
-struct GbSampleStats { unsigned distinct, f1, f2, adjacent, nulls, empties, n_cand, pad; };
+struct GbSampleStats { unsigned distinct, f1, f2, adjacent, nulls, empties, n_cand, pad; unsigned long long pairs; };
 struct GbCandidate { uint64_t key; uint64_t mult; };
 __global__ void k_gb_estimate(const void* keys, const uint32_t* key_validity, int key_dtype, int64_t n, int64_t m, uint64_t* scratch, unsigned* mult, uint64_t cap, int shift, GbSampleStats* stats) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) {
@@ -495,19 +496,22 @@ __global__ void k_gb_estimate(const void* keys, const uint32_t* key_validity, in
         }
     }
 }
-// f1 / f2 (keys sampled exactly once / twice) and the heavy-hitter candidates (multiplicity >= hot_thr)
+// f1 / f2 (keys sampled exactly once / twice), pairs and the heavy-hitter candidates (multiplicity >= hot_thr)
 __global__ void k_gb_estimate_stats(const uint64_t* scratch, const unsigned* mult, int64_t cap, unsigned hot_thr, GbSampleStats* stats, GbCandidate* cand) {
     unsigned f1 = 0, f2 = 0;
+    unsigned long long pairs = 0;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (int64_t)gridDim.x * blockDim.x) {
         const unsigned c = mult[i];
         f1 += c == 1; f2 += c == 2;
+        if (c > 1) pairs += (unsigned long long)c * (c - 1);
         if (c >= hot_thr) {
             const unsigned at = atomicAdd(&stats->n_cand, 1u);
             if (at < GB_CAND_MAX) { cand[at].key = scratch[i]; cand[at].mult = c; }
         }
     }
     f1 = __reduce_add_sync(0xffffffffu, f1); f2 = __reduce_add_sync(0xffffffffu, f2);
-    if (lane_id() == 0) { if (f1) atomicAdd(&stats->f1, f1); if (f2) atomicAdd(&stats->f2, f2); }
+    for (int o = 16; o > 0; o >>= 1) pairs += __shfl_xor_sync(0xffffffffu, pairs, o);
+    if (lane_id() == 0) { if (f1) atomicAdd(&stats->f1, f1); if (f2) atomicAdd(&stats->f2, f2); if (pairs) atomicAdd(&stats->pairs, pairs); }
 }
 __global__ void k_fill_u64(uint64_t* p, uint64_t v, int64_t n) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = v;
@@ -1017,7 +1021,7 @@ void GroupByState::build_hot_list(const void* cand_v, int n_cand, bool null_hot,
 }
 
 uint64_t GroupByState::choose_cap(const DevCol& key, int64_t n_total) {
-    double G, G_raw, G_upper = 0;
+    double G, G_raw, G_upper = 0, f2 = 0;
     if (expected_groups > 0) G = G_raw = (double)expected_groups;
     else {
         const int64_t n = key.len, m = std::min<int64_t>(n, 65536);
@@ -1067,9 +1071,15 @@ uint64_t GroupByState::choose_cap(const DevCol& key, int64_t n_total) {
         // new key the table would need distinct + (f1/m) * rows entries.  Heavy-tailed keys sit between the two
         // (Zipf(1.1): Chao 2.6e5, truth 1e6), so the table takes whatever the L2 budget allows up to that bound.
         G_upper = std::min(nt, (double)st.distinct + (double)st.f1 / (double)m * nt);
+        // sum over groups of (rows in the group)^2 in this batch: a group of c rows shows up s times in a sample of a share
+        // q = m / n of the rows, E[s (s - 1)] = q^2 c (c - 1)
+        if (m > 0) { const double q = (double)m / (double)n; f2 = (double)n + (double)st.pairs / (q * q); }
         build_hot_list(cand, (int)std::min<unsigned>(st.n_cand, GB_CAND_MAX), st.nulls >= hot_thr, st.empties >= hot_thr, (double)m);
     }
     est_groups = (int64_t)(G_raw * 1.25) + 2;      // for the shared-memory plan (overflow falls through to the global table)
+    // floor by Cauchy-Schwarz, F2 >= n^2 / groups: a strided sample of sorted or clustered keys sees a group at most once
+    // (pairs ~ 0) however many rows it has
+    est_f2 = f2 > 0 ? std::max(f2, (double)key.len * (double)key.len / (double)est_groups) : 0.0;
     const double lf_knob = knob_double("BL_K5_LF", 60.0) / 100.0, lf = (lf_knob > 0.05 && lf_knob < 0.95) ? lf_knob : 0.6;
     uint64_t c = pow2_at_least(G / lf);       // load factor <= 0.6 by default
     // keep the table inside L2 when a load factor <= 0.85 allows it: past ~55 % of L2 the REDs miss and the

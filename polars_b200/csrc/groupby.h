@@ -95,6 +95,7 @@ struct GroupByState {
     int64_t merged_rows = 0;     // partial-aggregate rows merged in (bounds the group count together with rows_seen)
     int64_t est_groups = 0;      // sampled / hinted cardinality; selects the shared-memory plan
     double sample_adjacent = 0;  // sampled fraction of rows whose successor carries the same key (skew / sortedness)
+    double est_f2 = 0;           // sampled sum over groups of (rows in the group)^2 in the batch (0: not sampled); sizes K5r's bucket streams
     GbHotDev hot{};              // heavy hitters found in the sample (rows == 0: none)
     double hot_share = 0;        // sampled share of the hottest key
     DevPtr hot_buf;

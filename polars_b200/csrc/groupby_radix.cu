@@ -4,7 +4,8 @@
 // hashing.rs:116-167, which ALSO partitions the keys by hash_to_partition before it builds one table per partition, and
 // agg_sum/mean/min/max, aggregations/mod.rs:486-1018).  groupby.cu aggregates with L2 atomics into one open-addressing
 // table; once that table outgrows L2 every RED becomes a DRAM read-modify-write.  This plan moves the rows instead of the atomics:
-//   pass 0  k_gbr_hist      rows per bucket (bucket = top bits of table_hash(key): the slot function of the L2 plan)
+//   pass 0  k_gbr_hist      rows per bucket (bucket = top bits of table_hash(key): the slot function of the L2 plan), only
+//                           when the sample cannot size the bucket streams (consume_radix: "exact" sizing)
 //   pass 1  k_gbr_scatter   every CTA sorts a 2048-row tile by bucket in shared memory as ROW-MAJOR records
 //                           [key, v0, v1, ...] and writes each (tile, bucket) run with ONE cp.async.bulk (TMA)
 //                           shared->global copy (runs padded to an even record count with a GB_EMPTY-key record so both
@@ -22,8 +23,9 @@
 // While the L2 plan's table stays in L2 this plan loses to it (64-bit shared-memory atomics on random slots cost several
 // SM cycles per row), so it is only taken when the L2 plan's table would exceed the L2 budget.
 // Restrictions (anything else stays on the L2 plan): no validity bitmaps, no first-row tracking, <= 4 value columns,
-// no heavy hitters in the sample.  Exact for any input: bucket capacities come from the exact histogram; a bucket with
-// more groups than its shared-memory table holds raises the status flag and the caller redoes the batch on the L2 plan.
+// no heavy hitters in the sample.  Exact for any input: a bucket that outgrows the stream the sample sized for it raises
+// status 2 and the caller redoes the batch with capacities from the exact histogram; a bucket with more groups than its
+// shared-memory table holds raises status 1 and the caller redoes the batch on the L2 plan.
 #include <algorithm>
 #include <cstdlib>
 
@@ -37,15 +39,20 @@ namespace plb {
 constexpr int GBR_THREADS = 512;      // pass 1: 2048-row tiles (bulk stores) / 4096-row tiles (many buckets: longer runs per bucket)
 constexpr int GBR_MAX_LOGB = 13;
 constexpr int GBR_NCW = 31, GBR_NCT = GBR_NCW * 32;                                    // pass 2: 31 consumer warps + 1 producer warp
+// pass 1: a reservation that would end past its bucket's stream (R.cap records) stores nothing and sets status 2; pass 2
+// then returns at entry and the caller redoes the batch with exact sizing.  The bound is a kernel parameter rather than
+// off[p + 1] - off[p]: two more loads per reservation made ptxas spill in k_gbr_scatter_wc<3, 8, *>.
+constexpr unsigned GBR_NO_ROOM = 0xFFFFFFFFu;
 
 struct GbRadixDev {
     uint64_t* recs;                 // record streams, bucket b at recs + off[b] * roww
     const unsigned long long* off;  // first record of bucket b (even; a multiple of GBR_WC_F for the write-combining scatter)
     unsigned* cursor;               // records written to bucket b so far (pads included)
-    unsigned* counts;               // pass 0: rows of bucket b
+    unsigned* counts;               // pass 0 (exact sizing): rows of bucket b
     int logB, roww;
     uint64_t* special;              // accumulator row of the GB_EMPTY-key group: [len, words...] (RED target; rare rows only)
-    int* status;
+    unsigned cap;                   // records of every bucket stream (sample sizing); ~0u: exact sizing, whose streams hold their rows by construction
+    int* status;                    // 1: a bucket's pass-2 table overflowed; 2: a bucket's record stream overflowed (pass 1)
 };
 
 // gb_load_pair of rows r0, r0 + 1 with a bounds check against n (rows past the end read as 0)
@@ -76,19 +83,27 @@ __global__ void __launch_bounds__(512) k_gbr_hist(const void* __restrict__ keys,
     __syncthreads();
     for (int i = threadIdx.x; i < B; i += blockDim.x) if (h_s[i]) atomicAdd(&counts[i], h_s[i]);
 }
-// bucket capacities -> exclusive offsets, one CTA.  Worst-case padding: `pad_each` records for each of up to `pad_units`
-// writers that touch the bucket (tile runs: one per tile; write-combining: F - 1 per CTA), rounded up to `align` records.
-__global__ void __launch_bounds__(1024) k_gbr_offsets(const unsigned* __restrict__ counts, int B, unsigned long long pad_units, unsigned pad_each, unsigned align,
-                                                      unsigned long long* __restrict__ off, unsigned* __restrict__ cursor) {
+// records of a bucket stream for `rows` rows: worst-case padding, `pad_each` records for each of up to `pad_units` writers
+// that touch the bucket (tile runs: one per tile; write-combining: F - 1 per CTA), rounded up to `align` records so that
+// every stream starts 16-byte (even) / 32-byte (F) aligned
+__host__ __device__ __forceinline__ unsigned long long gbr_stream_records(unsigned long long rows, unsigned long long pad_units, unsigned pad_each, unsigned align) {
+    rows += (rows < pad_units ? rows : pad_units) * pad_each;
+    return (rows + align - 1) & ~(unsigned long long)(align - 1);
+}
+// set-up of pass 1, one CTA: exclusive stream offsets from the exact row counts of k_gbr_hist (counts != nullptr) or from
+// `rows` rows for every bucket; zero cursors and status; the identities of the special row (a redone batch starts afresh)
+__global__ void __launch_bounds__(1024) k_gbr_offsets(const __grid_constant__ GbLayout L, const unsigned* __restrict__ counts, unsigned long long rows, int B, unsigned long long pad_units,
+                                                      unsigned pad_each, unsigned align, unsigned long long* __restrict__ off, unsigned* __restrict__ cursor, uint64_t* __restrict__ special, int* __restrict__ status) {
     __shared__ unsigned long long wsum[32];
     __shared__ unsigned long long carry_s;
-    if (threadIdx.x == 0) carry_s = 0;
+    if (threadIdx.x == 0) { carry_s = 0; *status = 0; special[0] = 0; }
+    if (threadIdx.x < (unsigned)L.n_words) special[1 + threadIdx.x] = L.init[threadIdx.x];
     __syncthreads();
     const unsigned lane = lane_id(), warp = threadIdx.x >> 5;
     for (int base = 0; base < B; base += 1024) {
         const int i = base + threadIdx.x;
         unsigned long long c = 0;
-        if (i < B) { c = counts[i]; c += (c < pad_units ? c : pad_units) * pad_each; c = (c + align - 1) & ~(unsigned long long)(align - 1); cursor[i] = 0; }   // every stream starts 16-byte (even) / 32-byte (F) aligned
+        if (i < B) { c = gbr_stream_records(counts ? counts[i] : rows, pad_units, pad_each, align); cursor[i] = 0; }
         unsigned long long x = c;
         for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= (unsigned)o) x += y; }
         if (lane == 31) wsum[warp] = x;
@@ -185,7 +200,9 @@ __global__ void __launch_bounds__(GBR_THREADS) k_gbr_scatter(const __grid_consta
             if (p < B) {
                 const unsigned c = hist[p], cp = BULK ? ((c + 1u) & ~1u) : c;
                 start[p] = run;
-                gpos[p] = cp ? atomicAdd(&R.cursor[p], cp) : 0u;
+                unsigned g = cp ? atomicAdd(&R.cursor[p], cp) : 0u;
+                if (g + cp > R.cap) { *R.status = 2; g = GBR_NO_ROOM; }
+                gpos[p] = g;
                 run += cp;
             }
         }
@@ -225,15 +242,15 @@ __global__ void __launch_bounds__(GBR_THREADS) k_gbr_scatter(const __grid_consta
         if (BULK) {
             for (int p = tid; p < B; p += THREADS) {
                 const unsigned c = hist[p], cp = (c + 1u) & ~1u;
-                if (cp) bulk_s2g(R.recs + (R.off[p] + gpos[p]) * ROWW, stage + (size_t)start[p] * ROWW, cp * ROWW * 8);
+                if (cp && gpos[p] != GBR_NO_ROOM) bulk_s2g(R.recs + (R.off[p] + gpos[p]) * ROWW, stage + (size_t)start[p] * ROWW, cp * ROWW * 8);
             }
             bulk_commit();
         } else {
             const unsigned total = start[B - 1] + hist[B - 1];
             for (unsigned w = tid; w < total * ROWW; w += THREADS) {
                 const unsigned row = w / ROWW, c = w - row * ROWW;
-                const unsigned p = sp[row];
-                R.recs[(R.off[p] + gpos[p] + (row - start[p])) * ROWW + c] = stage[w];
+                const unsigned p = sp[row], g = gpos[p];
+                if (g != GBR_NO_ROOM) R.recs[(R.off[p] + g + (row - start[p])) * ROWW + c] = stage[w];
             }
             __syncthreads();
         }
@@ -331,7 +348,9 @@ __global__ void __launch_bounds__(GBR_WC_THREADS, 2) k_gbr_scatter_wc(const __gr
 #pragma unroll
                 for (int q = 0; q < 4; q++) {
                     const int p = p0 + q * THREADS + tid;
-                    if (g[q] != NONE) bulk_s2g(R.recs + (R.off[p] + g[q]) * ROWW, buf + (size_t)p * CH, CH * 8);
+                    if (g[q] == NONE) continue;
+                    if (g[q] + F <= R.cap) bulk_s2g(R.recs + (R.off[p] + g[q]) * ROWW, buf + (size_t)p * CH, CH * 8);
+                    else *R.status = 2;
                 }
             }
             bulk_commit();
@@ -349,7 +368,8 @@ __global__ void __launch_bounds__(GBR_WC_THREADS, 2) k_gbr_scatter_wc(const __gr
         for (unsigned i = f; i < F; i++) buf[(size_t)p * CH + i * ROWW] = GB_EMPTY;
         fence_async_smem();
         const unsigned g = atomicAdd(&R.cursor[p], (unsigned)F);
-        bulk_s2g(R.recs + (R.off[p] + g) * ROWW, buf + (size_t)p * CH, CH * 8);
+        if (g + F <= R.cap) bulk_s2g(R.recs + (R.off[p] + g) * ROWW, buf + (size_t)p * CH, CH * 8);
+        else *R.status = 2;
     }
     bulk_commit();
     bulk_wait0();
@@ -370,6 +390,7 @@ __global__ void __launch_bounds__(1024) k_gbr_agg(const __grid_constant__ GbLayo
     __shared__ uint64_t full[NST], empty[NST];
     __shared__ unsigned s_used, s_base;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, B = 1 << R.logB;
+    if (*R.status == 2) return;                 // pass 1 overflowed a stream (every warp, the producer's included): the batch is redone
     if (tid == 0) { for (int s = 0; s < NST; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], GBR_NCW); } mbar_fence_init(); }
     __syncthreads();
     if (warp == GBR_NCW) {                      // producer warp: keeps the ring full across bucket boundaries
@@ -563,8 +584,20 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
     auto with_scatter_form = [&](auto f) { with_key_form(key.dtype, [&](auto e, auto c) { with_at_least<1, 2, 3, 4, 5>(roww, [&](auto w) { f(e, c, w); }); }); };
     int wc_grid = 0;
     if (wc) with_scatter_form([&](auto e, auto c, auto w) { wc_grid = scatter_wc_grid<decltype(w)::value, decltype(e)::value, decltype(c)::value>(B); });
-    const int64_t pad_rows = bulk ? std::min<int64_t>(n, (int64_t)B * ntiles) : wc ? std::min<int64_t>(n, (int64_t)B * wc_grid) * (GBR_WC_F - 1) : 0;
-    const int64_t rec_rows = n + pad_rows + (wc ? GBR_WC_F : 2) * (int64_t)B + 16;
+    // worst-case padding of a bucket stream (gbr_stream_records): one record per tile for the runs, F - 1 per CTA for the
+    // write-combining buffers, none for the coalesced store
+    const unsigned long long pad_units = wc ? (unsigned long long)wc_grid : (unsigned long long)ntiles;
+    const unsigned pad_each = wc ? GBR_WC_F - 1 : bulk ? 1u : 0u, align = wc ? GBR_WC_F : 2u;
+    // Bucket streams.  Sample sizing: every bucket gets room for n / B + 5 sqrt(F2 / B) rows (+ padding), F2 = est_f2 (the
+    // sum over groups of their rows squared).  A group lands in bucket b with probability 1 / B, so the rows of b have mean
+    // n / B and variance ~F2 / B; at z = 5 one bucket overflows with probability ~3e-7, one of 1024 with ~3e-4, and an
+    // overflow costs one redone batch.  Taken when the margin is at most half the mean (streams <= 1.5 n records + padding).
+    // Otherwise, and when nothing was sampled, exact sizing up front: k_gbr_hist counts every bucket's rows, one more read
+    // of the keys.  C2 (1e8 rows, 1e6 uniform keys: F2 ~1.01e10, 1024 buckets): 97,656 + 15,700 rows per bucket.
+    const double mean = (double)n / B, margin = 5.0 * std::sqrt(est_f2 / B);
+    unsigned long long bucket_rows = est_f2 > 0 && margin <= 0.5 * mean ? (unsigned long long)std::ceil(mean + margin) : 0;      // 0: exact sizing
+    const int64_t exact_rows = n + std::min<int64_t>(n, (int64_t)B * (int64_t)pad_units) * pad_each + (int64_t)align * B + 16;
+    int64_t rec_rows = bucket_rows ? (int64_t)B * (int64_t)gbr_stream_records(bucket_rows, pad_units, pad_each, align) + 16 : exact_rows;
     DevPtr recs, ctl;
     try {
         recs = dev_alloc((size_t)rec_rows * roww * 8);
@@ -577,39 +610,48 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
     R.special = reinterpret_cast<uint64_t*>(cp); cp += (size_t)(1 + GB_MAX_WORDS) * 8;
     R.counts = reinterpret_cast<unsigned*>(cp); cp += (size_t)B * 4;
     R.cursor = reinterpret_cast<unsigned*>(cp);
-    dev_memset(ctl->p, 0, ctl->bytes);
-    {   // identities of the special accumulator row
-        uint64_t h[1 + GB_MAX_WORDS]; h[0] = 0; for (int w = 0; w < L.n_words; w++) h[1 + w] = L.init[w];
-        PLB_CUDA(cudaMemcpyAsync(R.special, h, (size_t)(1 + L.n_words) * 8, cudaMemcpyHostToDevice, ctx().stream));
-        PLB_CUDA(cudaStreamSynchronize(ctx().stream));      // h lives on this frame
-    }
-    dev_memset(status->p, 0, 4);
-    with_key_form(key.dtype, [&](auto e, auto c) {
-        PLB_LAUNCH("k5r_histogram", (k_gbr_hist<decltype(e)::value, decltype(c)::value>), ctx().sm_count * 4, 512, (size_t)B * 4, key.v(), n, logB, R.counts);
-    });
-    if (wc) PLB_LAUNCH("k5r_offsets", k_gbr_offsets, 1, 1024, 0, R.counts, B, (unsigned long long)wc_grid, (unsigned)(GBR_WC_F - 1), (unsigned)GBR_WC_F, const_cast<unsigned long long*>(R.off), R.cursor);
-    else PLB_LAUNCH("k5r_offsets", k_gbr_offsets, 1, 1024, 0, R.counts, B, (unsigned long long)ntiles, bulk ? 1u : 0u, 2u, const_cast<unsigned long long*>(R.off), R.cursor);
-    with_scatter_form([&](auto e, auto c, auto w) {
-        constexpr int E = decltype(e)::value, C = decltype(c)::value, ROWW = decltype(w)::value;
-        if (wc) PLB_LAUNCH("k5r_scatter", (k_gbr_scatter_wc<ROWW, E, C>), wc_grid, GBR_WC_THREADS, gbr_wc_smem(B, ROWW), Lb, Bt, R);
-        else launch_scatter<ROWW, E, C>(Lb, Bt, R, bulk);
-    });
     // dense output, sized by a generous bound on the group count (overflow -> status -> fall back)
     const int64_t Gb = std::max<int64_t>(1024, std::min<int64_t>(n + 1, 3 * est_groups + (1 << 16)));
     dense.keys = dev_alloc((size_t)Gb * 8); dense.first = dev_alloc((size_t)Gb * 4); dense.len = dev_alloc((size_t)Gb * 4);
     dense.words = dev_alloc((size_t)Gb * 8 * std::max(L.n_words, 1)); dense.ctl = dev_alloc(16); dense.Gb = Gb;
-    const long long ctl_init[2] = {0, -1};
-    PLB_CUDA(cudaMemcpyAsync(dense.ctl->p, ctl_init, 16, cudaMemcpyHostToDevice, ctx().stream));
     GbDenseDev D{as<uint64_t>(dense.keys), as<uint32_t>(dense.first), as<uint32_t>(dense.len), as<uint64_t>(dense.words), Gb, as<unsigned long long>(dense.ctl)};
-    with_at_least<1, 2, 3, 4, 5>(roww, [&](auto w) { launch_agg<decltype(w)::value>(Lb, Bt, R, D, S); });
-    PLB_LAUNCH("k5r_special", k_gbr_append_special, 1, 32, 0, R.special, L.n_words, D, as<int>(status));
-    const int st = read_scalar(as<int>(status));      // also orders ctl_init / recs lifetimes
-    if (getenv("BL_K5_DEBUG")) fprintf(stderr, "[k5r] rows=%lld est_groups=%lld buckets=%d slots=%u bulk=%d store=%s status=%d\n", (long long)n, (long long)est_groups, B, S, (int)bulk,
-                                      bulk ? "runs" : wc ? "wc" : "coalesced", st);
-    if (st != 0) { dense = GbDense{}; dev_memset(status->p, 0, 4); return false; }
-    dense.ready = true;
-    rows_seen = n;
-    return true;
+    for (;;) {
+        const unsigned long long cap = bucket_rows ? gbr_stream_records(bucket_rows, pad_units, pad_each, align) : 0;      // records per bucket stream
+        R.cap = cap ? (unsigned)cap : ~0u;
+        if (!bucket_rows) {
+            dev_memset(R.counts, 0, (size_t)B * 4);
+            with_key_form(key.dtype, [&](auto e, auto c) {
+                PLB_LAUNCH("k5r_histogram", (k_gbr_hist<decltype(e)::value, decltype(c)::value>), ctx().sm_count * 4, 512, (size_t)B * 4, key.v(), n, logB, R.counts);
+            });
+        }
+        PLB_LAUNCH("k5r_setup", k_gbr_offsets, 1, 1024, 0, L, bucket_rows ? nullptr : R.counts, bucket_rows, B, pad_units, pad_each, align,
+                   const_cast<unsigned long long*>(R.off), R.cursor, R.special, R.status);
+        with_scatter_form([&](auto e, auto c, auto w) {
+            constexpr int E = decltype(e)::value, C = decltype(c)::value, ROWW = decltype(w)::value;
+            if (wc) PLB_LAUNCH("k5r_scatter", (k_gbr_scatter_wc<ROWW, E, C>), wc_grid, GBR_WC_THREADS, gbr_wc_smem(B, ROWW), Lb, Bt, R);
+            else launch_scatter<ROWW, E, C>(Lb, Bt, R, bulk);
+        });
+        dev_memset(dense.ctl->p, 0, 8); dev_memset(static_cast<char*>(dense.ctl->p) + 8, 0xFF, 8);      // {0, -1}
+        with_at_least<1, 2, 3, 4, 5>(roww, [&](auto w) { launch_agg<decltype(w)::value>(Lb, Bt, R, D, S); });
+        PLB_LAUNCH("k5r_special", k_gbr_append_special, 1, 32, 0, R.special, L.n_words, D, as<int>(status));
+        const int st = read_scalar(as<int>(status));      // also orders the recs lifetime
+        if (getenv("BL_K5_DEBUG"))
+            fprintf(stderr, "[k5r] rows=%lld est_groups=%lld buckets=%d slots=%u bulk=%d store=%s sizing=%s cap=%llu status=%d\n", (long long)n, (long long)est_groups, B, S, (int)bulk,
+                    bulk ? "runs" : wc ? "wc" : "coalesced", bucket_rows ? "sample" : "exact", cap, st);
+        if (st == 2 && bucket_rows) {       // a bucket outgrew its sampled stream: once more with exact sizing
+            bucket_rows = 0;
+            if (exact_rows > rec_rows) {
+                recs.reset();
+                try { recs = dev_alloc((size_t)exact_rows * roww * 8); } catch (const Error&) { cudaGetLastError(); dense = GbDense{}; dev_memset(status->p, 0, 4); return false; }
+                R.recs = as<uint64_t>(recs); rec_rows = exact_rows;
+            }
+            continue;
+        }
+        if (st != 0) { dense = GbDense{}; dev_memset(status->p, 0, 4); return false; }
+        dense.ready = true;
+        rows_seen = n;
+        return true;
+    }
 }
 
 }  // namespace plb
