@@ -372,6 +372,51 @@ enum { BL_IE_LT = 0, BL_IE_LE = 1, BL_IE_GT = 2, BL_IE_GE = 3 };
 bl_status bl_ie_join(const bl_column* left_on, const bl_column* right_on, const int32_t* ops, int32_t n_pred,
                      int32_t how, int32_t out_location, bl_column* out_left_idx, bl_column* out_right_idx);
 
+/* ---- window functions  (expr.over(partition_by, order_by), polars-expr/src/expressions/window.rs; cum_* cum_agg.rs) ---- */
+enum { BL_CUM_SUM = 32, BL_CUM_PROD = 33, BL_CUM_MIN = 34, BL_CUM_MAX = 35, BL_CUM_COUNT = 36, BL_SHIFT = 37 };
+typedef struct bl_over_op {
+    int32_t kind;             /* BL_AGG_* (broadcast to the group's rows) or BL_CUM_* / BL_SHIFT */
+    int32_t reverse;          /* BL_CUM_*: scan from the partition's last row */
+    int64_t periods;          /* BL_SHIFT */
+    const bl_column* values;  /* one chunk; NULL only for BL_AGG_LEN */
+    bl_agg_param param;       /* BL_AGG_QUANTILE */
+} bl_over_op;
+/* mapping_strategy "group_to_rows": outs[i] has one row per input row, in input row order.
+ * Partitions: the partition_by columns (numeric or string, one chunk for a numeric column, flags 0) group rows exactly as
+ * bl_groupby_agg_keys / bl_groupby_agg_strings do (a null key is its own group, floats -0 == +0 and NaN == NaN, strings by
+ * their bytes).  n_partition_by == 0: all rows form one partition (over() without keys, and the plain cum_sum() of a column).
+ * Order inside a partition: row order (GroupsIdx), or with order_by (NULL or ONE key, numeric, Bool or string, its flags
+ * BL_SORT_DESCENDING | BL_SORT_NULLS_LAST) each partition's rows stably sorted by that key in the total order (NaN greatest),
+ * ties in row order (update_groups_sort_by, polars-expr/src/expressions/sortby.rs:57-100).
+ * Aggregations (every BL_AGG_* kind, BL_AGG_WITH_DDOF, BL_AGG_N_UNIQUE, MEDIAN, QUANTILE through `param`): the group's value
+ * on each of its rows, with the output dtypes, validity and errors of bl_groupby_agg_params.  order_by only changes what FIRST,
+ * LAST, VAR / STD (Welford order) and float SUM / MEAN (sequential order) see: with order_by every aggregation is folded over
+ * the sorted rows.  A Bool value column takes only BL_AGG_COUNT and BL_AGG_LEN.
+ * Scans (polars-ops/src/series/ops/cum_agg.rs): a null input gives a null output and leaves the state unchanged (:14-53);
+ * `reverse` scans from the partition's last row.
+ *   BL_CUM_SUM    Int8/16, UInt8/16 -> Int64, Bool -> UInt32, 32/64-bit integers keep their dtype and wrap; Float64 in f64;
+ *                 Float32 accumulates in f64 and rounds every output to f32 (det_sum_to_f64, :38-45; :302-333)
+ *   BL_CUM_PROD   Bool, Int8..UInt32 -> Int64; Int64 / UInt64 keep their dtype and wrap; floats keep theirs (:261-285)
+ *   BL_CUM_MIN / BL_CUM_MAX  keep the dtype; floats ignore NaN (the initial state is NaN, an all-NaN prefix gives NaN,
+ *                 :78-112; the float impl of min_ignore_nan / max_ignore_nan is <$T>::min / <$T>::max,
+ *                 polars-utils/src/min_max.rs:87-108, which returns the non-NaN argument).  Between two equal values
+ *                 (only -0.0 and +0.0 differ in bits) MIN keeps the later in scan order and MAX the earlier: this tie rule
+ *                 is this library's statement, not read from the reference (IEEE minNum / maxNum leave the sign of a zero
+ *                 result open).  Bool: BL_ERR_UNSUPPORTED.
+ *   BL_CUM_COUNT  UInt32, never null, any dtype: valid values in [partition start, row], reverse [row, partition end] (:428-466)
+ *   BL_SHIFT      the value `periods` positions earlier in partition order (later for periods < 0), null when that position
+ *                 is outside the partition or null; keeps the dtype.  Bool: BL_ERR_UNSUPPORTED.
+ * Exactness: integer scans, CUM_MIN / MAX, CUM_COUNT and SHIFT are bit-identical to the reference.  Float CUM_SUM / CUM_PROD
+ * run a parallel scan: at the k-th row of a partition's scan |dev - ref| <= 2 (k - 1) u sum_{i<=k} |a_i| (products:
+ * 2 (k - 1) u |ref| while no partial product overflows or underflows), 0 for exactly summable values.  Under
+ * bl_set_deterministic(1) each partition is folded sequentially in scan order and floats are bit-identical too.
+ * Errors: BL_ERR_INVALID for value / key columns of different lengths, an unknown kind, partition flags != 0, unknown order_by
+ * flags, a missing value column, no column at all to give the row count; BL_ERR_UNSUPPORTED for the dtypes above, Bool
+ * partition columns, more than 2^31 - 1 rows when a sort is needed (partitioned scans, shifts, anything with order_by), and
+ * the aggregation errors of bl_groupby_agg_params.  One order_by key per call: the caller sorts by several keys itself. */
+bl_status bl_over(const bl_sort_key* partition_by, int32_t n_partition_by, const bl_sort_key* order_by, const bl_over_op* ops, int32_t n_ops,
+                  int32_t out_location, bl_column* outs);
+
 /* ---- K6: radix hash partition (multi-GPU exchange step) --------------------------------- */
 /* partition id = hash_to_partition(dirty_hash(key), n_partitions)
  *              = ((key * 0x55fbfd6bfc5458e9 mod 2^64) * n_partitions) >> 64   (hashing.rs:62-69,132-142),

@@ -871,6 +871,85 @@ def ie_join(left_on, right_on, ops, how: str = "inner", left_cols: Sequence = ()
     return take(left_cols, li), take(right_cols, ri)
 
 
+CUMS = {"cum_sum": 32, "cum_prod": 33, "cum_min": 34, "cum_max": 35, "cum_count": 36}
+SHIFT = 37
+
+
+class BlOverOp(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("reverse", C.c_int32), ("periods", C.c_int64), ("values", C.POINTER(BlColumn)), ("param", BlAggParam)]
+
+
+def _over_op(kind: str, column, options: dict, keep: list) -> BlOverOp:
+    """one (kind, column, options) tuple of over() -> a bl_over_op"""
+    if not isinstance(kind, str):
+        raise ValueError(f"an over() kind is a string, not {kind!r}")
+    options = dict(options or {})
+    name = kind.partition(":")[0]
+    allowed = {"reverse"} if name in CUMS else {"periods"} if name == "shift" else set()
+    unknown = set(options) - allowed
+    if unknown:
+        raise ValueError(f"{kind!r} takes no option(s) {', '.join(sorted(unknown))}")
+    if name in CUMS:
+        code = CUMS[name]
+    elif name == "shift":
+        code = SHIFT
+    elif name in AGGS or name == "quantile":
+        code = _agg_kind(kind)
+    else:
+        raise ValueError(f"unknown over() kind {kind!r}")
+    param = _agg_param(kind) if name == "quantile" else None
+    if column is None and name != "len":
+        raise ValueError(f"{kind!r} needs a value column")
+    ptr = None
+    if column is not None:
+        c = _as_col(column)
+        st = c.struct()
+        keep.append((c, st))
+        ptr = C.pointer(st)
+    return BlOverOp(code, int(bool(options.get("reverse", False))), int(options.get("periods", 1)), ptr, BlAggParam(*(param or (0.0, 0)), 0))
+
+
+def over(ops: Sequence, partition_by=(), order_by=None, descending: bool = False, nulls_last: bool = False, location: int = HOST):
+    """bl_over: window functions with one output row per input row (`expr.over(partition_by, order_by=...)`).
+    ops: (kind, column, options) tuples; kind is an aggregation of AGGS ("sum" ... "quantile:<q>:<method>", broadcast to the
+    rows of each partition) or "cum_sum" / "cum_prod" / "cum_min" / "cum_max" / "cum_count" (option `reverse`) or "shift"
+    (option `periods`, default 1).  partition_by: key columns (numeric, StringColumn / DeviceStringColumn); none = one
+    partition.  order_by: one key column (numeric, Bool or string) with `descending` / `nulls_last`.
+    Returns one output per op, as gather returns them."""
+    if isinstance(partition_by, (np.ndarray, Column, OutColumn, StringColumn, DeviceStringColumn)):
+        partition_by = [partition_by]
+    partition_by = list(partition_by or [])
+    if isinstance(order_by, list):
+        if len(order_by) != 1:
+            raise ValueError(f"over() takes one order_by column, not {len(order_by)}")
+        order_by = order_by[0]
+    if not ops:
+        raise ValueError("over() needs at least one operation")
+    keep = []
+    descs = []
+    for op in ops:
+        if not isinstance(op, tuple) or len(op) not in (2, 3):
+            raise ValueError(f"an over() operation is (kind, column[, options]), not {op!r}")
+        descs.append(_over_op(op[0], op[1], op[2] if len(op) == 3 else {}, keep))
+    parr = (BlSortKey * max(len(partition_by), 1))(*[_by_key(k, keep) for k in partition_by])
+    okey = None
+    if order_by is not None:
+        okey = _by_key(order_by, keep)
+        okey.flags = (SORT_DESCENDING if descending else 0) | (SORT_NULLS_LAST if nulls_last else 0)
+    oarr = (BlOverOp * len(descs))(*descs)
+    outs = (BlColumn * len(descs))()
+    _check(lib().bl_over(parr if partition_by else None, C.c_int32(len(partition_by)), C.byref(okey) if okey is not None else None, oarr,
+                         C.c_int32(len(descs)), C.c_int32(location), outs))
+    return _finish(list(outs), location)
+
+
+def cum_agg(kind: str, column, reverse: bool = False, location: int = HOST):
+    """The plain cum_sum() / cum_prod() / cum_min() / cum_max() / cum_count() of a column: over() with no partition."""
+    if kind not in CUMS:
+        raise ValueError(f"unknown cumulative kind {kind!r} (one of {', '.join(CUMS)})")
+    return over([(kind, column, {"reverse": reverse})], location=location)[0]
+
+
 def hash_partition(key, payload: Sequence, n_partitions: int, location: int = HOST):
     k = _as_col(key)
     ps = [_as_col(p) for p in payload]

@@ -158,6 +158,13 @@ DevCol op_cast_small_int(const DevCol& in, int to_dtype, bool bits);
 DevCol op_group_first_ids(const DevCol& key);
 DevCol op_pack_keys(const std::vector<DevCol>& keys);
 void op_group_tuples(const DevCol& key, DevCol& out_first, DevCol& out_offsets, DevCol& out_all);
+// op_group_tuples from the row -> first-row group ids; ids is sorted in place (on return ids[p] is the group of out_all[p])
+void op_group_tuples_ids(DevCol& ids, DevCol& out_first, DevCol& out_offsets, DevCol& out_all);
+// groups of an order whose group ids ascend: out_offsets = the positions where sorted_ids changes (+ n), out_first = all there
+void op_group_offsets(const DevCol& sorted_ids, const DevCol& all, DevCol& out_first, DevCol& out_offsets);
+// the sequential per-group folds of op_group_by_exact over given groups: group g owns rows all[offsets[g] .. offsets[g+1])
+void op_group_fold(const DevCol& offsets, const DevCol& all, const std::vector<int>& kinds, const std::vector<const DevCol*>& values, std::vector<DevCol>& outs,
+                   const bl_agg_param* params = nullptr);
 // deterministic mode: GroupsIdx + one sequential fold per group in the reference's order (groupby_exact.cu)
 // params[i] (quantile, method) is read where kinds[i] == BL_AGG_QUANTILE; nullptr = none given
 void op_group_by_exact(const DevCol& key, const std::vector<int>& kinds, const std::vector<const DevCol*>& values, DevCol& out_first, std::vector<DevCol>& outs,
@@ -176,6 +183,12 @@ DevCol op_arg_sort(const std::vector<DevCol>& by, const std::vector<int>& flags,
 void op_sort(const std::vector<DevCol>& by, const std::vector<int>& flags, const std::vector<DevCol>& cols, int64_t limit, std::vector<DevCol>& outs);
 void iota_u32(uint32_t* p, int64_t n, uint32_t base);
 inline int bits_for(uint64_t max_value) { int b = 1; while (b < 32 && (max_value >> b)) b++; return b; }   // digits the radix sort has to look at
+
+// window functions (window.cu): one output row per input row for every op; values NULL only for BL_AGG_LEN
+struct OverOp { int kind = 0; bool reverse = false; int64_t periods = 0; const DevCol* values = nullptr; bl_agg_param param{0.5, BL_QUANTILE_LINEAR, 0}; };
+void check_over_op(int kind_word, int value_dtype);      // BL_ERR_INVALID / BL_ERR_UNSUPPORTED of one op (value_dtype < 0: none)
+std::vector<DevCol> op_over(const std::vector<DevCol>& partition_by, const DevCol* order_key, int order_flags, const std::vector<OverOp>& ops, int64_t n);
+int over_scan_dtype(int kind, int dtype);      // output dtype of BL_CUM_* / BL_SHIFT
 
 struct JoinResult { DevCol left, right; };
 JoinResult op_hash_join(const DevCol& left, const DevCol& right, int how, bool nulls_equal, int maintain_order);

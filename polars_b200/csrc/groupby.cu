@@ -1680,7 +1680,13 @@ DevCol op_pack_keys(const std::vector<DevCol>& keys) {
 }
 
 void op_group_tuples(const DevCol& key, DevCol& out_first, DevCol& out_offsets, DevCol& out_all) {
-    const int64_t n = key.len;
+    PLB_REQUIRE(key.len <= 0x7FFFFFFFll, BL_ERR_UNSUPPORTED, "group_tuples: more than 2^31-1 rows");
+    DevCol ids = op_group_first_ids(key);
+    op_group_tuples_ids(ids, out_first, out_offsets, out_all);
+}
+
+void op_group_tuples_ids(DevCol& ids, DevCol& out_first, DevCol& out_offsets, DevCol& out_all) {
+    const int64_t n = ids.len;
     PLB_REQUIRE(n <= 0x7FFFFFFFll, BL_ERR_UNSUPPORTED, "group_tuples: more than 2^31-1 rows");
     out_all = make_col(BL_UINT32, n, false);
     if (n == 0) {
@@ -1689,16 +1695,19 @@ void op_group_tuples(const DevCol& key, DevCol& out_first, DevCol& out_offsets, 
         dev_memset(out_offsets.values->p, 0, 4);
         return;
     }
-    DevCol ids = op_group_first_ids(key);
-    DevPtr gid = ids.values;
     iota_u32(as<uint32_t>(out_all.values), n, 0);
-    sort_pairs_u32(as<uint32_t>(gid), as<uint32_t>(out_all.values), n, bits_for((uint64_t)n));
+    sort_pairs_u32(as<uint32_t>(ids.values), as<uint32_t>(out_all.values), n, bits_for((uint64_t)n));
+    op_group_offsets(ids, out_all, out_first, out_offsets);
+}
+
+void op_group_offsets(const DevCol& sorted_ids, const DevCol& all, DevCol& out_first, DevCol& out_offsets) {
+    const int64_t n = sorted_ids.len;
     DevCol starts = make_col(BL_BOOL, n, false);
     const int64_t n_round = (n + 31) / 32 * 32;
-    PLB_LAUNCH("k5_run_starts", k_run_starts, grid_for(n_round, 256, 16), 256, 0, as<uint32_t>(gid), n, n_round, as<uint32_t>(starts.values));
+    PLB_LAUNCH("k5_run_starts", k_run_starts, grid_for(n_round, 256, 16), 256, 0, as<uint32_t>(sorted_ids.values), n, n_round, as<uint32_t>(starts.values));
     DevCol pos = make_col(BL_UINT32, n, false);
     iota_u32(as<uint32_t>(pos.values), n, 0);
-    std::vector<DevCol> in{pos, out_all}, outv;
+    std::vector<DevCol> in{pos, all}, outv;
     op_filter(in, starts, outv);
     const int64_t G = outv[0].len;
     out_first = outv[1];

@@ -139,13 +139,11 @@ static int exact_out_dtype(int kind, int in_dtype) {
     }
 }
 
-// key: the (single, possibly packed) key column; values[i] == nullptr for LEN.  Groups come in first-occurrence order.
-// MEDIAN / QUANTILE go to op_group_quantiles (quantile.cu), one call per distinct value column.
-void op_group_by_exact(const DevCol& key, const std::vector<int>& kinds, const std::vector<const DevCol*>& values, DevCol& out_first, std::vector<DevCol>& outs,
-                       const bl_agg_param* params) {
-    std::vector<double> qs(kinds.size(), 0.5);
-    std::vector<int> methods(kinds.size(), BL_QUANTILE_LINEAR);      // MEDIAN = quantile(0.5, Linear) (aggregations/mod.rs:385-408)
-    for (size_t i = 0; i < kinds.size(); i++) {      // argument errors before any device work
+// argument errors of a GroupsIdx call, before any device work; qs / methods: each aggregation's quantile parameters
+static void exact_args(const std::vector<int>& kinds, const bl_agg_param* params, std::vector<double>& qs, std::vector<int>& methods) {
+    qs.assign(kinds.size(), 0.5);
+    methods.assign(kinds.size(), BL_QUANTILE_LINEAR);      // MEDIAN = quantile(0.5, Linear) (aggregations/mod.rs:385-408)
+    for (size_t i = 0; i < kinds.size(); i++) {
         const int kind = kinds[i] & 0xFFFF;
         PLB_REQUIRE(kind >= BL_AGG_SUM && kind <= BL_AGG_QUANTILE && kind != BL_AGG_N_UNIQUE, BL_ERR_INVALID, "group_by: unknown aggregation kind");
         if (kind != BL_AGG_QUANTILE) continue;
@@ -156,9 +154,27 @@ void op_group_by_exact(const DevCol& key, const std::vector<int>& kinds, const s
         PLB_REQUIRE(params[i].quantile >= 0.0 && params[i].quantile <= 1.0, BL_ERR_UNSUPPORTED, "group_by: quantile " + std::to_string(params[i].quantile) + " is outside [0, 1]");
         qs[i] = params[i].quantile; methods[i] = params[i].method;
     }
+}
+
+// key: the (single, possibly packed) key column; values[i] == nullptr for LEN.  Groups come in first-occurrence order.
+void op_group_by_exact(const DevCol& key, const std::vector<int>& kinds, const std::vector<const DevCol*>& values, DevCol& out_first, std::vector<DevCol>& outs,
+                       const bl_agg_param* params) {
+    std::vector<double> qs;
+    std::vector<int> methods;
+    exact_args(kinds, params, qs, methods);
     DevCol offsets, all;
     op_group_tuples(key, out_first, offsets, all);
-    const int64_t G = out_first.len;
+    op_group_fold(offsets, all, kinds, values, outs, params);
+}
+
+// Each group folded sequentially in the order of its row list (row order for op_group_by_exact, the window's order_by order
+// for bl_over).  MEDIAN / QUANTILE go to op_group_quantiles (quantile.cu), one call per distinct value column.
+void op_group_fold(const DevCol& offsets, const DevCol& all, const std::vector<int>& kinds, const std::vector<const DevCol*>& values, std::vector<DevCol>& outs,
+                   const bl_agg_param* params) {
+    std::vector<double> qs;
+    std::vector<int> methods;
+    exact_args(kinds, params, qs, methods);
+    const int64_t G = offsets.len - 1;
     outs.assign(kinds.size(), DevCol());
     std::vector<bool> done(kinds.size(), false);
     for (size_t i = 0; i < kinds.size(); i++) {

@@ -140,7 +140,7 @@ static void release_inputs(SeriesExport* inputs, size_t n) {
     }
 }
 
-enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT };
+enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER };
 
 // ---- kwargs ----------------------------------------------------------------------------------------
 // register_plugin_function(kwargs={...}) pickles the dict (py-polars/src/polars/plugins.py:100-115) and the caller hands
@@ -203,7 +203,7 @@ static int join_how_of(int op) { return op; }
 static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, const Kwargs& kw, SeriesExport* ret) {
     std::lock_guard<std::recursive_mutex> lk(ctx().mu);
     PLB_REQUIRE(n >= 1, BL_ERR_INVALID, "plugin: no input series");
-    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
+    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
     std::vector<std::vector<bl_column>> chunks(n);
     std::vector<DevCol> in;
     for (size_t i = 0; i < n; i++) { int dt; chunks[i] = input_chunks(inputs[i], &dt); in.push_back(import_column(chunks[i].data(), (int)chunks[i].size())); }
@@ -245,6 +245,17 @@ static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, co
             bl_column h; export_column(perm, BL_HOST, &h);
             fill_array(array, h);
             fill_schema(schema, name, format_of(BL_UINT32));
+        } else if (kind == P_OVER) {
+            // inputs: the values, then the partition keys (none: one partition) -> one row per input row (bl_over).
+            // kwargs: reverse (bool), periods (int, default 1)
+            check_over_op(op, in[0].dtype);
+            OverOp o;
+            o.kind = op; o.reverse = kw.get("reverse", 0) != 0; o.periods = (int64_t)kw.get("periods", 1); o.values = &in[0];
+            const std::vector<DevCol> parts(in.begin() + 1, in.end());
+            const DevCol r = op_over(parts, nullptr, 0, {o}, in[0].len)[0];
+            bl_column h; export_column(r, BL_HOST, &h);
+            fill_array(array, h);
+            fill_schema(schema, name, format_of(r.dtype));
         } else if (kind == P_GROUP) {
             // inputs: key_0 .. key_{k-1}, value (LEN: keys only)  ->  struct {key, key_1, ..., agg}, groups in first-occurrence order
             const bool is_len = op == BL_AGG_LEN;
@@ -335,6 +346,7 @@ static void field_entry(PluginOp kind, int op, const ArrowSchema* fields, size_t
         case P_ARITH: fill_schema(out, name, format_of((op == BL_OP_TRUE_DIV && dt >= 0 && dt <= BL_UINT64) ? BL_FLOAT64 : (dt < 0 ? BL_INT64 : dt))); break;
         case P_CMP: fill_schema(out, name, "b"); break;
         case P_SORT: fill_schema(out, name, format_of(BL_UINT32)); break;
+        case P_OVER: fill_schema(out, name, format_of(over_scan_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_FILTER: case P_GATHER: fill_schema(out, name, format_of(dt < 0 ? BL_INT64 : dt)); break;
         case P_GROUP: {
             const size_t nk = op == BL_AGG_LEN ? n : (n > 0 ? n - 1 : 0);
@@ -401,4 +413,10 @@ PLUGIN(join_full_idx, P_JOIN, BL_JOIN_FULL)
 PLUGIN(join_semi_idx, P_JOIN, BL_JOIN_SEMI)
 PLUGIN(join_anti_idx, P_JOIN, BL_JOIN_ANTI)
 PLUGIN(arg_sort, P_SORT, 0)                     /* kwargs: descending, nulls_last (bool or bitmask); inputs = by columns */
+PLUGIN(cum_sum, P_OVER, BL_CUM_SUM)             /* kwargs: reverse; inputs = values, then partition keys */
+PLUGIN(cum_prod, P_OVER, BL_CUM_PROD)
+PLUGIN(cum_min, P_OVER, BL_CUM_MIN)
+PLUGIN(cum_max, P_OVER, BL_CUM_MAX)
+PLUGIN(cum_count, P_OVER, BL_CUM_COUNT)
+PLUGIN(shift, P_OVER, BL_SHIFT)                 /* kwargs: periods (default 1) */
 }
