@@ -417,6 +417,65 @@ typedef struct bl_over_op {
 bl_status bl_over(const bl_sort_key* partition_by, int32_t n_partition_by, const bl_sort_key* order_by, const bl_over_op* ops, int32_t n_ops,
                   int32_t out_location, bl_column* outs);
 
+/* ---- rolling windows  (expr.rolling_*(window_size, min_samples, center), polars-compute/src/rolling; .over() as bl_over) ---- */
+enum { BL_ROLLING_SUM = 40, BL_ROLLING_MEAN = 41, BL_ROLLING_MIN = 42, BL_ROLLING_MAX = 43, BL_ROLLING_VAR = 44, BL_ROLLING_STD = 45 };
+typedef struct bl_rolling_op {
+    int32_t kind;            /* BL_ROLLING_* */
+    int32_t center;
+    int64_t window_size;     /* >= 1 */
+    int64_t min_samples;     /* 0 .. window_size */
+    int32_t ddof;            /* VAR / STD, 0 .. 255 */
+    int32_t reserved;        /* 0 */
+    const bl_column* values; /* one chunk */
+} bl_rolling_op;
+/* outs[i] has one row per input row, in input row order.  partition_by / order_by: exactly bl_over's meaning and checks; each
+ * partition is evaluated on its own, in partition order, and the results go back to the rows.
+ * Window of the k-th position of a partition of m positions (w = window_size; polars-compute/src/rolling/mod.rs:72-87):
+ *   trailing  [k - w + 1, k], center  [k - (w - r), k + r) with r = ceil(w / 2); both clipped to [0, m) (det_offsets /
+ *   det_offsets_center, saturating_sub at the start, min(len, .) at the end).
+ * Validity: null when the window holds fewer than min_samples non-null values (is_valid, rolling/sum.rs:219-221,
+ * nulls/mod.rs:46-98; create_validity mod.rs:89-127 only nulls a subset of those rows).  The C ABI takes min_samples
+ * explicitly (the Python default window_size is the binding's, polars-python/src/expr/rolling.rs:19).
+ *   BL_ROLLING_SUM   Int8/16, UInt8/16 -> Int64, Bool -> UInt32, 32/64-bit integers keep their dtype and wrap
+ *                    (polars-time/src/chunkedarray/rolling_window/dispatch.rs:284-312).  Floats keep theirs; only finite values
+ *                    are summed, non-finite ones are counted: only +inf gives +inf, only -inf gives -inf, any other mix NaN
+ *                    (rolling/sum.rs:68-108).  A window without non-null values sums to 0 (valid when min_samples == 0).
+ *   BL_ROLLING_MEAN  Float32 for Float32, Float64 for everything else (to_float, dispatch.rs:238-249): the sum in f64 with the
+ *                    same non-finite rule, cast to the output type, divided by the non-null count in that type
+ *                    (rolling/mean.rs:98-108); a window without non-null values is null whatever min_samples.
+ *   BL_ROLLING_MIN / BL_ROLLING_MAX  keep the dtype; NaN propagates (any NaN in the window gives NaN), and among equal values
+ *                    (-0.0 / +0.0) the earliest in the window wins (ArgMinMaxWindow, rolling/arg_min_max.rs: a later value
+ *                    replaces the deque's tail only when strictly better; MinPropagateNan / MaxPropagateNan,
+ *                    polars-utils/src/min_max.rs:91-98,155-186).  A window without non-null values is null.  Bool: unsupported.
+ *   BL_ROLLING_VAR / BL_ROLLING_STD  Float32 for Float32, Float64 otherwise, computed in f64 (VarState,
+ *                    polars-compute/src/moment.rs:90-129): null when the non-null count <= ddof; a negative variance is 0;
+ *                    any non-finite value in the window gives NaN (its validity still follows the count, rolling/moment.rs:
+ *                    163-206).  Float32: (float)var; STD is sqrt of that value in the output type (dispatch.rs:565-576).
+ * Temporal columns: pass their physical Int64 and convert the result back.
+ * Exactness: integer SUM, every MIN / MAX, every validity bit and the non-finite class (NaN / +inf / -inf) of every window
+ * holding a non-finite value are bit-identical to the reference.  Not reproduced: a window of finite values whose sum
+ * overflows gives +-inf here, where the reference's Kahan state (f32 for Float32 SUM) overflows to inf and then to NaN
+ * (err_add = inf, inf + -inf).  Finite float windows are reduced as two sequential runs joined by one combine (DESIGN.md §13); against
+ * the EXACT value of a window of k non-null values a_i (u the unit roundoff of f64, u_o of the output type):
+ *   SUM   |dev - exact| <= 1.01 (k - 1) u sum|a_i| + u_o |exact|
+ *   MEAN  |dev - exact| <= (1.01 (k - 1) u sum|a_i| + u_o |sum|) / k + 2 u_o |exact|
+ *   VAR   |dev - exact| <= 4.04 (k + 2) u sum (a_i - mean)^2 (1 + k mean^2 / sum (a_i - mean)^2)^(1/2) / (k - ddof) + u_o |exact|
+ *   STD   |dev - exact| <= sqrt(the VAR bound) + u_o |exact|
+ * These bound the distance to the exact window value, not to the reference's incremental Kahan / two-stack value, which
+ * depends on the history of the column.  Under bl_set_deterministic(1), float SUM / MEAN / VAR / STD replay the reference's
+ * state machines (SumWindow's Kahan add / sub and its reset when a window starts at or past the previous end; MomentWindow's
+ * two stacks and flip) sequentially per partition and are bit-identical.
+ * Plans (DESIGN.md §13), chosen from B = min(window_size, rows): B <= 128 runs one pass that stages each 1024-row tile and
+ * its halo in shared memory; larger B writes per-block prefix and suffix states to device memory (2 x rows x 16..32 bytes of
+ * scratch: 6.4 GB for VAR / STD over 1e8 rows) and its scans run ceil(rows / B) CTAs wide, so a window of a large share of
+ * the column (say 1e7 of 1e8 rows) uses only a few SMs.
+ * Errors: BL_ERR_INVALID for min_samples > window_size (dispatch.rs:42), a negative window_size or min_samples, ddof outside
+ * 0..255, reserved != 0, an unknown kind, a missing value column, columns of different lengths and bl_over's key errors;
+ * BL_ERR_UNSUPPORTED for window_size == 0, a Bool column for anything but SUM, Bool partition columns, more than 2^31 - 1
+ * rows with partitions or order_by and more than 2^32 - 1 rows otherwise. */
+bl_status bl_rolling(const bl_sort_key* partition_by, int32_t n_partition_by, const bl_sort_key* order_by, const bl_rolling_op* ops,
+                     int32_t n_ops, int32_t out_location, bl_column* outs);
+
 /* ---- K6: radix hash partition (multi-GPU exchange step) --------------------------------- */
 /* partition id = hash_to_partition(dirty_hash(key), n_partitions)
  *              = ((key * 0x55fbfd6bfc5458e9 mod 2^64) * n_partitions) >> 64   (hashing.rs:62-69,132-142),

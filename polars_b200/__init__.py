@@ -950,6 +950,87 @@ def cum_agg(kind: str, column, reverse: bool = False, location: int = HOST):
     return over([(kind, column, {"reverse": reverse})], location=location)[0]
 
 
+ROLLINGS = {"rolling_sum": 40, "rolling_mean": 41, "rolling_min": 42, "rolling_max": 43, "rolling_var": 44, "rolling_std": 45}
+
+
+class BlRollingOp(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("center", C.c_int32), ("window_size", C.c_int64), ("min_samples", C.c_int64), ("ddof", C.c_int32),
+                ("reserved", C.c_int32), ("values", C.POINTER(BlColumn))]
+
+
+def _rolling_op(kind: str, column, options: dict, keep: list) -> BlRollingOp:
+    """one (kind, column, options) tuple of rolling() -> a bl_rolling_op"""
+    if kind not in ROLLINGS:
+        raise ValueError(f"unknown rolling kind {kind!r} (one of {', '.join(ROLLINGS)})")
+    options = dict(options or {})
+    allowed = {"window_size", "min_samples", "center"} | ({"ddof"} if kind in ("rolling_var", "rolling_std") else set())
+    unknown = set(options) - allowed
+    if unknown:
+        raise ValueError(f"{kind!r} takes no option(s) {', '.join(sorted(unknown))}")
+    if "window_size" not in options:
+        raise ValueError(f"{kind!r} needs a window_size")
+    ws = options["window_size"]
+    ms = options.get("min_samples")
+    ms = ws if ms is None else ms
+    ddof = options.get("ddof", 1)
+    for name, v in (("window_size", ws), ("min_samples", ms), ("ddof", ddof)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+            raise ValueError(f"{kind!r}: {name} must be an integer, not {v!r}")
+    if ws < 1:
+        raise ValueError(f"{kind!r}: window_size must be at least 1, not {ws}")
+    if not 0 <= ms <= ws:
+        raise ValueError(f"{kind!r}: min_samples ({ms}) must be in 0..window_size ({ws})")
+    if not 0 <= ddof <= 255:
+        raise ValueError(f"{kind!r}: ddof must be in 0..255, not {ddof}")
+    if column is None:
+        raise ValueError(f"{kind!r} needs a value column")
+    c = _as_col(column)
+    st = c.struct()
+    keep.append((c, st))
+    return BlRollingOp(ROLLINGS[kind], int(bool(options.get("center", False))), int(ws), int(ms), int(ddof), 0, C.pointer(st))
+
+
+def rolling(ops: Sequence, partition_by=(), order_by=None, descending: bool = False, nulls_last: bool = False, location: int = HOST):
+    """bl_rolling: fixed-window rolling aggregations, one output row per input row (`expr.rolling_*(...)`, and with
+    partition_by / order_by `expr.rolling_*(...).over(partition_by, order_by=...)`).
+    ops: (kind, column, options) tuples; kind is one of ROLLINGS; options: window_size (required), min_samples (default
+    window_size), center (default False) and, for rolling_var / rolling_std, ddof (default 1).  partition_by / order_by /
+    descending / nulls_last as over() takes them.  Returns one output per op, as gather returns them."""
+    if isinstance(partition_by, (np.ndarray, Column, OutColumn, StringColumn, DeviceStringColumn)):
+        partition_by = [partition_by]
+    partition_by = list(partition_by or [])
+    if isinstance(order_by, list):
+        if len(order_by) != 1:
+            raise ValueError(f"rolling() takes one order_by column, not {len(order_by)}")
+        order_by = order_by[0]
+    if not ops:
+        raise ValueError("rolling() needs at least one operation")
+    keep = []
+    descs = []
+    for op in ops:
+        if not isinstance(op, tuple) or len(op) != 3:
+            raise ValueError(f"a rolling() operation is (kind, column, options), not {op!r}")
+        descs.append(_rolling_op(op[0], op[1], op[2], keep))
+    parr = (BlSortKey * max(len(partition_by), 1))(*[_by_key(k, keep) for k in partition_by])
+    okey = None
+    if order_by is not None:
+        okey = _by_key(order_by, keep)
+        okey.flags = (SORT_DESCENDING if descending else 0) | (SORT_NULLS_LAST if nulls_last else 0)
+    oarr = (BlRollingOp * len(descs))(*descs)
+    outs = (BlColumn * len(descs))()
+    _check(lib().bl_rolling(parr if partition_by else None, C.c_int32(len(partition_by)), C.byref(okey) if okey is not None else None, oarr,
+                            C.c_int32(len(descs)), C.c_int32(location), outs))
+    return _finish(list(outs), location)
+
+
+def rolling_agg(kind: str, column, window_size: int, min_samples=None, center: bool = False, ddof: int = 1, location: int = HOST):
+    """The plain rolling_sum() ... rolling_std() of a column: rolling() with no partition."""
+    opts = {"window_size": window_size, "min_samples": min_samples, "center": center}
+    if kind in ("rolling_var", "rolling_std"):
+        opts["ddof"] = ddof
+    return rolling([(kind, column, opts)], location=location)[0]
+
+
 def hash_partition(key, payload: Sequence, n_partitions: int, location: int = HOST):
     k = _as_col(key)
     ps = [_as_col(p) for p in payload]

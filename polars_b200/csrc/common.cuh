@@ -189,6 +189,23 @@ struct OverOp { int kind = 0; bool reverse = false; int64_t periods = 0; const D
 void check_over_op(int kind_word, int value_dtype);      // BL_ERR_INVALID / BL_ERR_UNSUPPORTED of one op (value_dtype < 0: none)
 std::vector<DevCol> op_over(const std::vector<DevCol>& partition_by, const DevCol* order_key, int order_flags, const std::vector<OverOp>& ops, int64_t n);
 int over_scan_dtype(int kind, int dtype);      // output dtype of BL_CUM_* / BL_SHIFT
+// the partition order shared by bl_over and bl_rolling (window.cu)
+struct OverOrder {
+    DevCol gid;               // row -> first row of its partition (UInt32)
+    DevCol perm, seg, offsets, inv;     // partition order, its group id per position, segment offsets (G + 1), inverse permutation
+    int64_t G = 0;
+};
+DevCol partition_ids(const std::vector<DevCol>& partition_by, int64_t n);      // row -> first row of its partition
+void build_order(OverOrder& o, const DevCol* order_key, int order_flags, bool need_inv);      // o.gid set by the caller
+DevCol import_key(const bl_sort_key& k, bool partition);      // partition: string codes; else: string ranks
+// argument checks of bl_over / bl_rolling (who: the message prefix); n: the common row count, -1 until a column sets it
+void set_window_len(const char* who, int64_t len, const std::string& what, int64_t& n);
+void check_window_keys(const char* who, const bl_sort_key* partition_by, int32_t n_partition_by, const bl_sort_key* order_by, int64_t& n);
+// rolling windows (rolling.cu)
+struct RollOp { int kind = 0; bool center = false; int64_t window_size = 1, min_samples = 1; int ddof = 1; const DevCol* values = nullptr; };
+void check_rolling_op(int kind, int center, int64_t window_size, int64_t min_samples, int ddof, int reserved, int value_dtype);
+int rolling_dtype(int kind, int dtype);
+std::vector<DevCol> op_rolling(const std::vector<DevCol>& partition_by, const DevCol* order_key, int order_flags, const std::vector<RollOp>& ops, int64_t n);
 
 struct JoinResult { DevCol left, right; };
 JoinResult op_hash_join(const DevCol& left, const DevCol& right, int how, bool nulls_equal, int maintain_order);

@@ -48,6 +48,10 @@ __host__ __device__ __forceinline__ int dtype_size_dev(int dt) {
 // ---- bitmaps (LSB-first; polars-arrow/src/bitmap/utils/mod.rs:42-46); device bitmaps are
 //      32-bit-word arrays with bit offset 0
 __device__ __forceinline__ bool bit_get(const uint32_t* bm, int64_t i) { return (bm[i >> 5] >> (i & 31)) & 1u; }
+// a value of column v at row r; BL_BOOL values are bit-packed (v NULL: every row counts as set, for CUM_COUNT)
+struct BoolBit { bool b; };
+template <typename In> __device__ __forceinline__ In load_in(const void* v, int64_t r) { return __ldg(reinterpret_cast<const In*>(v) + r); }
+template <> __device__ __forceinline__ BoolBit load_in<BoolBit>(const void* v, int64_t r) { return BoolBit{v == nullptr || bit_get(reinterpret_cast<const uint32_t*>(v), r)}; }
 
 // spread the 32 bits of x to the even bit positions of a 64-bit word
 __device__ __forceinline__ uint64_t spread_bits(uint32_t v) {

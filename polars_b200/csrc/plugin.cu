@@ -140,16 +140,17 @@ static void release_inputs(SeriesExport* inputs, size_t n) {
     }
 }
 
-enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER };
+enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER, P_ROLL };
 
 // ---- kwargs ----------------------------------------------------------------------------------------
 // register_plugin_function(kwargs={...}) pickles the dict (py-polars/src/polars/plugins.py:100-115) and the caller hands
 // the bytes through (plugin.rs:70-137; Rust plugins read them with serde-pickle).  The subset a flat {str: bool | int |
 // float | str | None} dict produces under protocols 2..5 is parsed here: PROTO FRAME EMPTY_DICT MARK (SHORT_)BINUNICODE
 // BININT BININT1 BININT2 LONG1 BINFLOAT NEWTRUE NEWFALSE NONE MEMOIZE BINPUT SETITEM SETITEMS STOP.
-struct Kwargs { std::vector<std::pair<std::string, double>> num; std::vector<std::pair<std::string, std::string>> str; std::vector<std::string> bools;
+struct Kwargs { std::vector<std::pair<std::string, double>> num; std::vector<std::pair<std::string, std::string>> str; std::vector<std::string> bools, nones;
     double get(const char* k, double dflt) const { for (auto& e : num) if (e.first == k) return e.second; return dflt; }
     bool is_bool(const char* k) const { for (auto& e : bools) if (e == k) return true; return false; }
+    bool is_none(const char* k) const { for (auto& e : nones) if (e == k) return true; return false; }
     std::string gets(const char* k, const char* dflt) const { for (auto& e : str) if (e.first == k) return e.second; return dflt; } };
 static Kwargs parse_kwargs(const uint8_t* p, size_t n) {
     Kwargs kw;
@@ -164,6 +165,7 @@ static Kwargs parse_kwargs(const uint8_t* p, size_t n) {
             if (st[j + 1].kind == 2) kw.str.push_back({st[j].s, st[j + 1].s});
             else kw.num.push_back({st[j].s, (st[j + 1].kind == 1 || st[j + 1].kind == 5) ? st[j + 1].num : 0.0});
             if (st[j + 1].kind == 5) kw.bools.push_back(st[j].s);
+            if (st[j + 1].kind == 0) kw.nones.push_back(st[j].s);
         }
         st.resize(from);
     };
@@ -203,7 +205,7 @@ static int join_how_of(int op) { return op; }
 static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, const Kwargs& kw, SeriesExport* ret) {
     std::lock_guard<std::recursive_mutex> lk(ctx().mu);
     PLB_REQUIRE(n >= 1, BL_ERR_INVALID, "plugin: no input series");
-    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
+    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER && kind != P_ROLL) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
     std::vector<std::vector<bl_column>> chunks(n);
     std::vector<DevCol> in;
     for (size_t i = 0; i < n; i++) { int dt; chunks[i] = input_chunks(inputs[i], &dt); in.push_back(import_column(chunks[i].data(), (int)chunks[i].size())); }
@@ -253,6 +255,21 @@ static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, co
             o.kind = op; o.reverse = kw.get("reverse", 0) != 0; o.periods = (int64_t)kw.get("periods", 1); o.values = &in[0];
             const std::vector<DevCol> parts(in.begin() + 1, in.end());
             const DevCol r = op_over(parts, nullptr, 0, {o}, in[0].len)[0];
+            bl_column h; export_column(r, BL_HOST, &h);
+            fill_array(array, h);
+            fill_schema(schema, name, format_of(r.dtype));
+        } else if (kind == P_ROLL) {
+            // inputs: the values, then the partition keys (none: one partition) -> one row per input row (bl_rolling).
+            // kwargs: window_size (int, required), min_samples (int; absent or None: window_size, as rolling_*(min_samples=None)
+            // means), center (bool), ddof (int, default 1)
+            const double ws = kw.is_none("window_size") ? std::nan("") : kw.get("window_size", std::nan(""));
+            PLB_REQUIRE(!std::isnan(ws), BL_ERR_INVALID, "plugin rolling_*: the `window_size` kwarg is required");
+            RollOp o;
+            o.kind = op; o.window_size = (int64_t)ws; o.min_samples = kw.is_none("min_samples") ? (int64_t)ws : (int64_t)kw.get("min_samples", ws); o.center = kw.get("center", 0) != 0;
+            o.ddof = (int)kw.get("ddof", 1); o.values = &in[0];
+            check_rolling_op(o.kind, o.center ? 1 : 0, o.window_size, o.min_samples, o.ddof, 0, in[0].dtype);
+            const std::vector<DevCol> parts(in.begin() + 1, in.end());
+            const DevCol r = op_rolling(parts, nullptr, 0, {o}, in[0].len)[0];
             bl_column h; export_column(r, BL_HOST, &h);
             fill_array(array, h);
             fill_schema(schema, name, format_of(r.dtype));
@@ -347,6 +364,7 @@ static void field_entry(PluginOp kind, int op, const ArrowSchema* fields, size_t
         case P_CMP: fill_schema(out, name, "b"); break;
         case P_SORT: fill_schema(out, name, format_of(BL_UINT32)); break;
         case P_OVER: fill_schema(out, name, format_of(over_scan_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
+        case P_ROLL: fill_schema(out, name, format_of(rolling_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_FILTER: case P_GATHER: fill_schema(out, name, format_of(dt < 0 ? BL_INT64 : dt)); break;
         case P_GROUP: {
             const size_t nk = op == BL_AGG_LEN ? n : (n > 0 ? n - 1 : 0);
@@ -419,4 +437,10 @@ PLUGIN(cum_min, P_OVER, BL_CUM_MIN)
 PLUGIN(cum_max, P_OVER, BL_CUM_MAX)
 PLUGIN(cum_count, P_OVER, BL_CUM_COUNT)
 PLUGIN(shift, P_OVER, BL_SHIFT)                 /* kwargs: periods (default 1) */
+PLUGIN(rolling_sum, P_ROLL, BL_ROLLING_SUM)     /* kwargs: window_size, min_samples, center, ddof; inputs = values, then partition keys */
+PLUGIN(rolling_mean, P_ROLL, BL_ROLLING_MEAN)
+PLUGIN(rolling_min, P_ROLL, BL_ROLLING_MIN)
+PLUGIN(rolling_max, P_ROLL, BL_ROLLING_MAX)
+PLUGIN(rolling_var, P_ROLL, BL_ROLLING_VAR)
+PLUGIN(rolling_std, P_ROLL, BL_ROLLING_STD)
 }

@@ -30,9 +30,6 @@ namespace plb {
 
 // ---------------------------------------------------------------------------------------------------- scan operators
 // S: the scan state; lift(x): a valid input as a state; combine(a, b): a earlier in scan order; out(s): the output value.
-struct BoolBit { bool b; };      // a BL_BOOL value column: bit-packed (NULL values: every row counts as set, for CUM_COUNT)
-template <typename In> __device__ __forceinline__ In load_in(const void* v, int64_t r) { return __ldg(reinterpret_cast<const In*>(v) + r); }
-template <> __device__ __forceinline__ BoolBit load_in<BoolBit>(const void* v, int64_t r) { return BoolBit{v == nullptr || bit_get(reinterpret_cast<const uint32_t*>(v), r)}; }
 
 // SUM: integers wrap in the output width (Int8/16, UInt8/16 arrive as Int64; Bool -> UInt32); Float32 accumulates in f64 and
 // rounds each output to f32 (det_sum_to_f64, cum_agg.rs:38-45)
@@ -331,12 +328,6 @@ int over_scan_dtype(int kind, int dt) {
     }
 }
 
-struct OverOrder {
-    DevCol gid;               // row -> first row of its partition (UInt32)
-    DevCol perm, seg, offsets, inv;     // partition order, its group id per position, segment offsets (G + 1), inverse permutation
-    int64_t G = 0;
-};
-
 template <class Op> static void launch_scan(const DevCol& v, const OverOrder* o, bool reverse, DevCol& out) {
     const int64_t n = v.len;
     if (n == 0) return;
@@ -452,7 +443,7 @@ static DevCol over_shift(const DevCol& v, const OverOrder* o, int64_t periods) {
 // The partition order, once per call.  Without order_by: op_group_tuples_ids (groups in first-occurrence order, rows
 // ascending).  With it: the stable arg_sort of (group id, order key), exactly update_groups_sort_by's per-group stable sort
 // (sortby.rs:57-100) with the groups in first-occurrence order; segments start where the group id changes.
-static void build_order(OverOrder& o, const DevCol* order_key, int order_flags, bool need_inv) {
+void build_order(OverOrder& o, const DevCol* order_key, int order_flags, bool need_inv) {
     const int64_t n = o.gid.len;
     DevCol first;
     if (!order_key) {
@@ -566,6 +557,15 @@ static int over_agg_dtype(int kind, int dt) {
     }
 }
 
+// row -> first row of its partition (UInt32); no partition columns: every row in partition 0
+DevCol partition_ids(const std::vector<DevCol>& partition_by, int64_t n) {
+    DevCol gid;
+    if (!partition_by.empty()) gid = op_group_first_ids(op_pack_keys(partition_by));
+    else { gid = make_col(BL_UINT32, n, false); dev_memset(gid.values->p, 0, (size_t)n * 4); }
+    gid.null_count = 0;
+    return gid;
+}
+
 // ops are checked by the caller (check_over_op) before any column is uploaded
 std::vector<DevCol> op_over(const std::vector<DevCol>& partition_by, const DevCol* order_key, int order_flags, const std::vector<OverOp>& ops, int64_t n) {
     std::vector<DevCol> vals(ops.size());
@@ -598,11 +598,7 @@ std::vector<DevCol> op_over(const std::vector<DevCol>& partition_by, const DevCo
     }
 
     OverOrder o;
-    if (any_agg || need_order) {
-        if (partitioned) o.gid = op_group_first_ids(op_pack_keys(partition_by));
-        else { o.gid = make_col(BL_UINT32, n, false); dev_memset(o.gid.values->p, 0, (size_t)n * 4); }
-        o.gid.null_count = 0;
-    }
+    if (any_agg || need_order) o.gid = partition_ids(partition_by, n);
     if (need_order) build_order(o, order_key, order_flags, need_inv);
     over_aggs(o, order_key != nullptr, ops, vals, outs);
     const OverOrder* order = need_order ? &o : nullptr;
@@ -635,10 +631,35 @@ static int64_t key_length(const bl_sort_key& k) {
     return n;
 }
 
-static DevCol import_key(const bl_sort_key& k, bool partition) {
+DevCol import_key(const bl_sort_key& k, bool partition) {
     if (k.column) return import_column(k.column, 1);
     DevStr s = import_string(k.strings, k.n_chunks);
     return partition ? op_string_codes(s, nullptr) : op_string_rank(s, false, nullptr);
+}
+
+void set_window_len(const char* who, int64_t len, const std::string& what, int64_t& n) {
+    if (n < 0) n = len;
+    PLB_REQUIRE(len == n, BL_ERR_INVALID, std::string(who) + ": " + what + " has " + std::to_string(len) + " rows, not " + std::to_string(n));
+}
+
+void check_window_keys(const char* who, const bl_sort_key* partition_by, int32_t n_partition_by, const bl_sort_key* order_by, int64_t& n) {
+    const std::string w0 = who;
+    PLB_REQUIRE(n_partition_by >= 0 && (n_partition_by == 0 || partition_by), BL_ERR_INVALID, w0 + ": n_partition_by > 0 needs partition_by");
+    auto check_key = [&](const bl_sort_key& k, const std::string& w) {
+        PLB_REQUIRE((k.column != nullptr) != (k.strings != nullptr), BL_ERR_INVALID, w + " must set exactly one of `column` and `strings`");
+        PLB_REQUIRE(k.strings == nullptr || k.n_chunks >= 1, BL_ERR_INVALID, w + ": a string column without chunks");
+        set_window_len(who, key_length(k), w, n);
+    };
+    for (int i = 0; i < n_partition_by; i++) {
+        const std::string w = "partition column " + std::to_string(i);
+        check_key(partition_by[i], w);
+        PLB_REQUIRE(partition_by[i].flags == 0, BL_ERR_INVALID, w0 + ": " + w + ": flags must be 0");
+        if (partition_by[i].column) PLB_REQUIRE(partition_by[i].column->dtype != BL_BOOL, BL_ERR_UNSUPPORTED, w0 + ": Boolean partition columns are outside the hot path");
+    }
+    if (order_by) {
+        check_key(*order_by, "the order_by column");
+        PLB_REQUIRE((order_by->flags & ~(BL_SORT_DESCENDING | BL_SORT_NULLS_LAST)) == 0, BL_ERR_INVALID, w0 + ": unknown order_by flags");
+    }
 }
 
 }  // namespace plb
@@ -651,29 +672,10 @@ bl_status bl_over(const bl_sort_key* partition_by, int32_t n_partition_by, const
                   int32_t out_location, bl_column* outs) {
     BL_TRY
     PLB_REQUIRE(n_ops >= 1 && ops && outs, BL_ERR_INVALID, "over: no operations or no outputs");
-    PLB_REQUIRE(n_partition_by >= 0 && (n_partition_by == 0 || partition_by), BL_ERR_INVALID, "over: n_partition_by > 0 needs partition_by");
     int64_t n = -1;
-    auto set_len = [&](int64_t len, const std::string& what) {
-        if (n < 0) n = len;
-        PLB_REQUIRE(len == n, BL_ERR_INVALID, "over: " + what + " has " + std::to_string(len) + " rows, not " + std::to_string(n));
-    };
-    auto check_key = [&](const bl_sort_key& k, const std::string& w) {
-        PLB_REQUIRE((k.column != nullptr) != (k.strings != nullptr), BL_ERR_INVALID, w + " must set exactly one of `column` and `strings`");
-        PLB_REQUIRE(k.strings == nullptr || k.n_chunks >= 1, BL_ERR_INVALID, w + ": a string column without chunks");
-        set_len(key_length(k), w);
-    };
-    for (int i = 0; i < n_partition_by; i++) {
-        const std::string w = "partition column " + std::to_string(i);
-        check_key(partition_by[i], w);
-        PLB_REQUIRE(partition_by[i].flags == 0, BL_ERR_INVALID, "over: " + w + ": flags must be 0");
-        if (partition_by[i].column) PLB_REQUIRE(partition_by[i].column->dtype != BL_BOOL, BL_ERR_UNSUPPORTED, "over: Boolean partition columns are outside the hot path");
-    }
-    if (order_by) {
-        check_key(*order_by, "the order_by column");
-        PLB_REQUIRE((order_by->flags & ~(BL_SORT_DESCENDING | BL_SORT_NULLS_LAST)) == 0, BL_ERR_INVALID, "over: unknown order_by flags");
-    }
+    check_window_keys("over", partition_by, n_partition_by, order_by, n);
     for (int i = 0; i < n_ops; i++) {
-        if (ops[i].values) set_len(ops[i].values->length, "value column " + std::to_string(i));
+        if (ops[i].values) set_window_len("over", ops[i].values->length, "value column " + std::to_string(i), n);
         else PLB_REQUIRE((ops[i].kind & 0xFFFF) == BL_AGG_LEN, BL_ERR_INVALID, "over: operation " + std::to_string(i) + " has no value column");
     }
     PLB_REQUIRE(n >= 0, BL_ERR_INVALID, "over: no column gives the number of rows");
