@@ -476,6 +476,62 @@ typedef struct bl_rolling_op {
 bl_status bl_rolling(const bl_sort_key* partition_by, int32_t n_partition_by, const bl_sort_key* order_by, const bl_rolling_op* ops,
                      int32_t n_ops, int32_t out_location, bl_column* outs);
 
+/* ---- time-based rolling windows  (expr.rolling_*_by(by, window_size, min_samples, closed), .over() as bl_rolling) ---- */
+enum { BL_CLOSED_RIGHT = 0, BL_CLOSED_LEFT = 1, BL_CLOSED_BOTH = 2, BL_CLOSED_NONE = 3 };
+typedef struct bl_rolling_by_op {
+    int32_t kind;            /* BL_ROLLING_* */
+    int32_t closed;          /* BL_CLOSED_* */
+    int64_t window_size;     /* P >= 1, in the physical unit of `by` */
+    int64_t min_samples;     /* >= 0 (no upper limit) */
+    int32_t ddof;            /* VAR / STD, 0 .. 255 */
+    int32_t reserved;        /* 0 */
+    const bl_column* values; /* one chunk */
+} bl_rolling_by_op;
+/* outs[i] has one row per input row, in input row order.  partition_by: bl_rolling's meaning and checks (each partition is
+ * evaluated on its own, as rolling_*_by(...).over(g) is).  Entry: rolling_agg_by, polars-time/src/chunkedarray/
+ * rolling_window/dispatch.rs:71-218.
+ * `by`: Int32, Int64, UInt32 or UInt64, one chunk, cast to Int64 as the reference does (:163-175).  A Date column is passed as
+ * its days times 86 400 000 000 (the reference casts it to Datetime(us)), a Datetime as its physical Int64, and P in the
+ * same unit: the Python binding parses durations ("5m", "1d", "3i") as Duration::add_ns / add_us / add_ms do
+ * (duration.rs:929-1045, sub-unit parts truncated).  Calendar durations (mo, q, y) and d / w on time-zone-aware columns are
+ * not expressible here.  Any other `by` dtype is BL_ERR_INVALID (:176-179); a UInt64 value >= 2^63 is BL_ERR_INVALID (the
+ * reference's non-strict cast makes it null and then fails on cont_slice().unwrap()).
+ * Order: each partition's rows sorted by `by`, ties in row order (a stable sort).  The reference arg-sorts an unsorted `by`
+ * with an unstable sort (SortOptions::default()); the tie order decides only the float summation order and which of -0.0 /
+ * +0.0 a MIN / MAX returns, which the reference leaves open.
+ * Window of the row at time t (group_by_values_iter_lookbehind, polars-time/src/windows/group_by.rs:247-326): the rows of
+ * its partition with lb < u <= t for BL_CLOSED_RIGHT, lb <= u <= t BOTH, lb <= u < t LEFT, lb < u < t NONE, lb = t - P
+ * (Bounds::is_member, bounds.rs:33-60).  Rows with equal times share one window (the duplicate fast path, :286-291): with
+ * RIGHT / BOTH it runs to the end of t's run of equal times; with LEFT / NONE it can be empty.  t - P is plain i64
+ * arithmetic and wraps near i64::MIN, as the reference's does in a release build: a wrapped lower bound is above every
+ * time, so such a row's window starts at its own run (empty for LEFT / NONE) and the reference's window start never moves
+ * back before the last such run of its partition.
+ * Output (rolling_apply_agg_window(_sorted), rolling_kernels/shared.rs:109-204): a window of fewer than min_samples rows,
+ * nulls included, is null; otherwise the kind's bl_rolling rule below (dtypes, validity by non-null count, non-finite
+ * classes, NaN-propagating MIN / MAX with the earliest of equal values, VarState) decides.  An empty window (min_samples
+ * = 0): SUM 0 (valid), MEAN / MIN / MAX / VAR / STD null.  A row whose `by` is null is null and belongs to no window
+ * (:101-129).  The Python defaults are min_samples 0 for rolling_sum_by and 1 for the others, closed "right", ddof 1.
+ * Exactness: as bl_rolling.  Integer SUM, MIN / MAX, validity and non-finite classes are bit-identical; the SUM / MEAN
+ * bounds of bl_rolling hold unchanged (they hold for any summation order of the window's k values).  A window is combined
+ * from at most five runs (prefix, suffix, two sparse-table states, or the in-block equivalents), each itself a combination
+ * of sequential runs, so the VAR bound takes the constant of DESIGN.md §14:
+ *   VAR   |dev - exact| <= 8.08 (k + 4) u sum (a_i - mean)^2 (1 + k mean^2 / sum (a_i - mean)^2)^(1/2) / (k - ddof) + u_o |exact|
+ *   STD   |dev - exact| <= sqrt(the VAR bound) + u_o |exact|
+ * Under bl_set_deterministic(1) float SUM / MEAN / VAR / STD replay the reference's window machines over the same windows,
+ * skipping update for the windows below min_samples; they are bit-identical when no two rows of a partition share a time
+ * (with ties, the reference's unstable order decides).
+ * Plans (DESIGN.md §14), chosen from the largest window W the bounds pass observes: W <= 128 runs one pass that stages each
+ * 1024-row tile and 128 positions on each side in shared memory (device memory: 8 bytes per row of window bounds); wider
+ * windows add blocks of 1024 positions with prefix / suffix states (2 x rows x 16..32 bytes: 6.4 GB for VAR over 1e8 rows)
+ * and a disjoint sparse table over the block totals (2 x ceil(log2(rows / 1024)) x rows / 1024 states: 106 MB for VAR over
+ * 1e8 rows).  The sort of the partitioned or unsorted form adds bl_over's.
+ * Errors: BL_ERR_INVALID for window_size <= 0, a negative min_samples, ddof outside 0..255, reserved != 0, an unknown kind or
+ * closed, a missing value or `by` column, the `by` dtypes and values above, columns of different lengths and bl_over's key
+ * errors; BL_ERR_UNSUPPORTED for a Bool column for anything but SUM, Bool partition columns, more than 2^31 - 1 rows when a
+ * sort is needed (partitions, a null or unsorted `by`) and more than 2^32 - 1 rows otherwise. */
+bl_status bl_rolling_by(const bl_sort_key* partition_by, int32_t n_partition_by, const bl_column* by, const bl_rolling_by_op* ops,
+                        int32_t n_ops, int32_t out_location, bl_column* outs);
+
 /* ---- K6: radix hash partition (multi-GPU exchange step) --------------------------------- */
 /* partition id = hash_to_partition(dirty_hash(key), n_partitions)
  *              = ((key * 0x55fbfd6bfc5458e9 mod 2^64) * n_partitions) >> 64   (hashing.rs:62-69,132-142),

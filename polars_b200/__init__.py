@@ -7,8 +7,10 @@ there is no CPU fallback and this package never imports oracle/.
 from __future__ import annotations
 
 import ctypes as C
+import datetime as _dt
 import json
 import os
+import re
 from typing import Sequence
 
 import numpy as np
@@ -1029,6 +1031,146 @@ def rolling_agg(kind: str, column, window_size: int, min_samples=None, center: b
     if kind in ("rolling_var", "rolling_std"):
         opts["ddof"] = ddof
     return rolling([(kind, column, opts)], location=location)[0]
+
+
+CLOSED = {"right": 0, "left": 1, "both": 2, "none": 3}
+_NS_OF = {"ns": 1, "us": 1_000, "ms": 1_000_000, "s": 1_000_000_000, "m": 60_000_000_000, "h": 3_600_000_000_000}
+_NS_DAY = 86_400_000_000_000
+_DIV_OF = {"ns": 1, "us": 1_000, "ms": 1_000_000}
+
+
+def window_size_in(window_size, unit) -> int:
+    """The window size P of rolling_*_by in the physical unit of `by`: an int is taken as it is; a duration string
+    ("30s", "1d12h", "3i") or a timedelta is converted as the reference's Duration::add_ns / add_us / add_ms do
+    (polars-time/src/windows/duration.rs:929-1045: weeks and days in whole units, the rest truncated to the unit).
+    unit: "ns" / "us" / "ms" for a temporal `by`, None for an integer one (which takes only "Ni" durations)."""
+    if isinstance(window_size, (int, np.integer)) and not isinstance(window_size, bool):
+        p = int(window_size)
+    else:
+        weeks = days = nsecs = index = 0
+        if isinstance(window_size, _dt.timedelta):
+            days, nsecs = window_size.days, (window_size.seconds * 1_000_000 + window_size.microseconds) * 1_000
+        elif isinstance(window_size, str):
+            parts = re.findall(r"(\d+)([a-z]+)", window_size)
+            if not parts or "".join(a + b for a, b in parts) != window_size:
+                raise ValueError(f"window_size {window_size!r} is not a duration such as '30s', '1d12h' or '3i'")
+            for num, u in parts:
+                k = int(num)
+                if u in ("mo", "q", "y"):
+                    raise ValueError(f"window_size {window_size!r}: calendar durations ({u}) are not supported on the device")
+                if u == "w":
+                    weeks += k
+                elif u == "d":
+                    days += k
+                elif u == "i":
+                    index += k
+                elif u in _NS_OF:
+                    nsecs += k * _NS_OF[u]
+                else:
+                    raise ValueError(f"window_size {window_size!r}: unknown unit {u!r}")
+            if index and (weeks or days or nsecs):
+                raise ValueError(f"window_size {window_size!r} mixes 'i' with temporal units")
+        else:
+            raise ValueError(f"window_size must be an int, a duration string or a timedelta, not {window_size!r}")
+        if unit is None:
+            if weeks or days or nsecs:
+                raise ValueError(f"an integer `by` column takes a window_size in 'i' units (such as '3i'), not {window_size!r}")
+            p = index
+        else:
+            if index:
+                raise ValueError(f"a temporal `by` column takes a temporal window_size, not {window_size!r}")
+            div = _DIV_OF[unit]
+            p = (weeks * 7 + days) * (_NS_DAY // div) + nsecs // div
+    if p <= 0:
+        raise ValueError(f"window_size must be strictly positive in the unit of `by` ({unit or 'i'}), got {p} from {window_size!r}")
+    if p >= 2 ** 63:
+        raise ValueError(f"window_size {window_size!r} does not fit in Int64 in the unit of `by`")
+    return p
+
+
+def _by_column(by):
+    """A `by` column -> (column for _as_col, unit).  numpy datetime64[ns|us|ms] keep their unit; datetime64[D] (Date)
+    becomes microseconds, as the reference casts Date to Datetime(us); NaT is null."""
+    if isinstance(by, np.ndarray) and by.dtype.kind == "M":
+        unit = np.datetime_data(by.dtype)[0]
+        if unit not in ("ns", "us", "ms", "D"):
+            raise ValueError(f"a datetime64[{unit}] `by` column is not supported (ns, us, ms or D)")
+        valid = ~np.isnat(by)
+        v = by.view(np.int64)
+        if unit == "D":
+            v, unit = np.where(valid, v, 0) * 86_400_000_000, "us"
+        return ((np.ascontiguousarray(v), valid) if not valid.all() else np.ascontiguousarray(v)), unit
+    return by, None
+
+
+class BlRollingByOp(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("closed", C.c_int32), ("window_size", C.c_int64), ("min_samples", C.c_int64), ("ddof", C.c_int32),
+                ("reserved", C.c_int32), ("values", C.POINTER(BlColumn))]
+
+
+def rolling_by(ops: Sequence, by, partition_by=(), location: int = HOST):
+    """bl_rolling_by: time-based rolling aggregations, one output row per input row (`expr.rolling_*_by(by, ...)`, and with
+    partition_by `expr.rolling_*_by(...).over(partition_by)`).
+    ops: (kind, column, options) tuples; kind is one of ROLLINGS; options: window_size (required: see window_size_in),
+    min_samples (default 0 for rolling_sum, 1 otherwise), closed ("right", "left", "both" or "none"; default "right") and,
+    for rolling_var / rolling_std, ddof (default 1).  by: an Int32 / Int64 / UInt32 / UInt64 column or a numpy datetime64
+    array.  Returns one output per op, as gather returns them."""
+    if isinstance(partition_by, (np.ndarray, Column, OutColumn, StringColumn, DeviceStringColumn)):
+        partition_by = [partition_by]
+    partition_by = list(partition_by or [])
+    if not ops:
+        raise ValueError("rolling_by() needs at least one operation")
+    byc, unit = _by_column(by)
+    keep = []
+    descs = []
+    for op in ops:
+        if not isinstance(op, tuple) or len(op) != 3:
+            raise ValueError(f"a rolling_by() operation is (kind, column, options), not {op!r}")
+        kind, column, options = op[0], op[1], dict(op[2] or {})
+        if kind not in ROLLINGS:
+            raise ValueError(f"unknown rolling kind {kind!r} (one of {', '.join(ROLLINGS)})")
+        allowed = {"window_size", "min_samples", "closed"} | ({"ddof"} if kind in ("rolling_var", "rolling_std") else set())
+        unknown = set(options) - allowed
+        if unknown:
+            raise ValueError(f"{kind!r} takes no option(s) {', '.join(sorted(unknown))}")
+        if "window_size" not in options:
+            raise ValueError(f"{kind!r} needs a window_size")
+        ws = window_size_in(options["window_size"], unit)
+        ms = options.get("min_samples")
+        ms = (0 if kind == "rolling_sum" else 1) if ms is None else ms
+        ddof = options.get("ddof", 1)
+        for name, v in (("min_samples", ms), ("ddof", ddof)):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+                raise ValueError(f"{kind!r}: {name} must be an integer, not {v!r}")
+        if ms < 0:
+            raise ValueError(f"{kind!r}: min_samples must not be negative, not {ms}")
+        if not 0 <= ddof <= 255:
+            raise ValueError(f"{kind!r}: ddof must be in 0..255, not {ddof}")
+        closed = options.get("closed", "right")
+        if closed not in CLOSED:
+            raise ValueError(f"{kind!r}: closed must be one of {', '.join(CLOSED)}, not {closed!r}")
+        if column is None:
+            raise ValueError(f"{kind!r} needs a value column")
+        c = _as_col(column)
+        st = c.struct()
+        keep.append((c, st))
+        descs.append(BlRollingByOp(ROLLINGS[kind], CLOSED[closed], ws, int(ms), int(ddof), 0, C.pointer(st)))
+    bc = _as_col(byc)
+    bst = bc.struct()
+    parr = (BlSortKey * max(len(partition_by), 1))(*[_by_key(k, keep) for k in partition_by])
+    oarr = (BlRollingByOp * len(descs))(*descs)
+    outs = (BlColumn * len(descs))()
+    _check(lib().bl_rolling_by(parr if partition_by else None, C.c_int32(len(partition_by)), C.byref(bst), oarr, C.c_int32(len(descs)),
+                               C.c_int32(location), outs))
+    return _finish(list(outs), location)
+
+
+def rolling_agg_by(kind: str, column, by, window_size, min_samples=None, closed: str = "right", ddof: int = 1, location: int = HOST):
+    """The plain rolling_sum_by() ... rolling_std_by() of a column: rolling_by() with no partition."""
+    opts = {"window_size": window_size, "min_samples": min_samples, "closed": closed}
+    if kind in ("rolling_var", "rolling_std"):
+        opts["ddof"] = ddof
+    return rolling_by([(kind, column, opts)], by, location=location)[0]
 
 
 def hash_partition(key, payload: Sequence, n_partitions: int, location: int = HOST):

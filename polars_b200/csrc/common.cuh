@@ -206,6 +206,10 @@ struct RollOp { int kind = 0; bool center = false; int64_t window_size = 1, min_
 void check_rolling_op(int kind, int center, int64_t window_size, int64_t min_samples, int ddof, int reserved, int value_dtype);
 int rolling_dtype(int kind, int dtype);
 std::vector<DevCol> op_rolling(const std::vector<DevCol>& partition_by, const DevCol* order_key, int order_flags, const std::vector<RollOp>& ops, int64_t n);
+// time-based rolling windows (rolling_by.cu)
+struct RollByOp { int kind = 0; int closed = 0; int64_t window_size = 1, min_samples = 1; int ddof = 1; const DevCol* values = nullptr; };
+void check_rolling_by_op(int kind, int closed, int64_t window_size, int64_t min_samples, int ddof, int reserved, int value_dtype);
+std::vector<DevCol> op_rolling_by(const std::vector<DevCol>& partition_by, const DevCol& by, const std::vector<RollByOp>& ops, int64_t n);
 
 struct JoinResult { DevCol left, right; };
 JoinResult op_hash_join(const DevCol& left, const DevCol& right, int how, bool nulls_equal, int maintain_order);

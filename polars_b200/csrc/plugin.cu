@@ -140,7 +140,7 @@ static void release_inputs(SeriesExport* inputs, size_t n) {
     }
 }
 
-enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER, P_ROLL };
+enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER, P_ROLL, P_ROLL_BY };
 
 // ---- kwargs ----------------------------------------------------------------------------------------
 // register_plugin_function(kwargs={...}) pickles the dict (py-polars/src/polars/plugins.py:100-115) and the caller hands
@@ -205,7 +205,7 @@ static int join_how_of(int op) { return op; }
 static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, const Kwargs& kw, SeriesExport* ret) {
     std::lock_guard<std::recursive_mutex> lk(ctx().mu);
     PLB_REQUIRE(n >= 1, BL_ERR_INVALID, "plugin: no input series");
-    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER && kind != P_ROLL) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
+    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER && kind != P_ROLL && kind != P_ROLL_BY) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
     std::vector<std::vector<bl_column>> chunks(n);
     std::vector<DevCol> in;
     for (size_t i = 0; i < n; i++) { int dt; chunks[i] = input_chunks(inputs[i], &dt); in.push_back(import_column(chunks[i].data(), (int)chunks[i].size())); }
@@ -270,6 +270,41 @@ static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, co
             check_rolling_op(o.kind, o.center ? 1 : 0, o.window_size, o.min_samples, o.ddof, 0, in[0].dtype);
             const std::vector<DevCol> parts(in.begin() + 1, in.end());
             const DevCol r = op_rolling(parts, nullptr, 0, {o}, in[0].len)[0];
+            bl_column h; export_column(r, BL_HOST, &h);
+            fill_array(array, h);
+            fill_schema(schema, name, format_of(r.dtype));
+        } else if (kind == P_ROLL_BY) {
+            // inputs: the values, the `by` column, then the partition keys -> one row per input row (bl_rolling_by).
+            // kwargs: window_size (int, required, in the physical unit of `by`), min_samples (int; absent or None: 0 for
+            // rolling_sum_by and 1 for the others, as the Python signatures default), closed ("right" / "left" / "both" /
+            // "none" or its BL_CLOSED_* code, default "right"), ddof (int, default 1)
+            PLB_REQUIRE(n >= 2, BL_ERR_INVALID, "plugin rolling_*_by: expected the values and the `by` column");
+            const double ws = kw.is_none("window_size") ? std::nan("") : kw.get("window_size", std::nan(""));
+            PLB_REQUIRE(!std::isnan(ws), BL_ERR_INVALID, "plugin rolling_*_by: the `window_size` kwarg is required");
+            const double ms = kw.is_none("min_samples") ? (op == BL_ROLLING_SUM ? 0 : 1) : kw.get("min_samples", op == BL_ROLLING_SUM ? 0 : 1);
+            // the kwargs carry numbers as doubles: only integers up to 2^53 arrive exactly
+            for (double v : {ws, ms})
+                PLB_REQUIRE(v == std::floor(v) && std::fabs(v) <= 9007199254740992.0, BL_ERR_INVALID, "plugin rolling_*_by: window_size and min_samples must be integers of at most 2^53");
+            // closed: "right" / "left" / "both" / "none", or its BL_CLOSED_* code
+            int closed = BL_CLOSED_RIGHT;
+            const std::string cs = kw.gets("closed", "");
+            if (!cs.empty()) {
+                const char* names[] = {"right", "left", "both", "none"};      // BL_CLOSED_RIGHT .. BL_CLOSED_NONE
+                closed = -1;
+                for (int c = 0; c < 4; c++) if (cs == names[c]) closed = c;
+                PLB_REQUIRE(closed >= 0, BL_ERR_INVALID, "plugin rolling_*_by: unknown closed '" + cs + "'");
+            } else {
+                const double c = kw.get("closed", BL_CLOSED_RIGHT);
+                PLB_REQUIRE(!kw.is_bool("closed") && c == std::floor(c) && c >= BL_CLOSED_RIGHT && c <= BL_CLOSED_NONE, BL_ERR_INVALID,
+                            "plugin rolling_*_by: closed must be 'right', 'left', 'both', 'none' or its code 0..3");
+                closed = (int)c;
+            }
+            RollByOp o;
+            o.kind = op; o.window_size = (int64_t)ws; o.min_samples = (int64_t)ms;
+            o.closed = closed; o.ddof = (int)kw.get("ddof", 1); o.values = &in[0];
+            check_rolling_by_op(o.kind, o.closed, o.window_size, o.min_samples, o.ddof, 0, in[0].dtype);
+            const std::vector<DevCol> parts(in.begin() + 2, in.end());
+            const DevCol r = op_rolling_by(parts, in[1], {o}, in[0].len)[0];
             bl_column h; export_column(r, BL_HOST, &h);
             fill_array(array, h);
             fill_schema(schema, name, format_of(r.dtype));
@@ -365,6 +400,7 @@ static void field_entry(PluginOp kind, int op, const ArrowSchema* fields, size_t
         case P_SORT: fill_schema(out, name, format_of(BL_UINT32)); break;
         case P_OVER: fill_schema(out, name, format_of(over_scan_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_ROLL: fill_schema(out, name, format_of(rolling_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
+        case P_ROLL_BY: fill_schema(out, name, format_of(rolling_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_FILTER: case P_GATHER: fill_schema(out, name, format_of(dt < 0 ? BL_INT64 : dt)); break;
         case P_GROUP: {
             const size_t nk = op == BL_AGG_LEN ? n : (n > 0 ? n - 1 : 0);
@@ -443,4 +479,10 @@ PLUGIN(rolling_min, P_ROLL, BL_ROLLING_MIN)
 PLUGIN(rolling_max, P_ROLL, BL_ROLLING_MAX)
 PLUGIN(rolling_var, P_ROLL, BL_ROLLING_VAR)
 PLUGIN(rolling_std, P_ROLL, BL_ROLLING_STD)
+PLUGIN(rolling_sum_by, P_ROLL_BY, BL_ROLLING_SUM)     /* kwargs: window_size, min_samples, closed (str or code), ddof; inputs = values, by, then partition keys */
+PLUGIN(rolling_mean_by, P_ROLL_BY, BL_ROLLING_MEAN)
+PLUGIN(rolling_min_by, P_ROLL_BY, BL_ROLLING_MIN)
+PLUGIN(rolling_max_by, P_ROLL_BY, BL_ROLLING_MAX)
+PLUGIN(rolling_var_by, P_ROLL_BY, BL_ROLLING_VAR)
+PLUGIN(rolling_std_by, P_ROLL_BY, BL_ROLLING_STD)
 }
