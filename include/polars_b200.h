@@ -532,6 +532,53 @@ typedef struct bl_rolling_by_op {
 bl_status bl_rolling_by(const bl_sort_key* partition_by, int32_t n_partition_by, const bl_column* by, const bl_rolling_by_op* ops,
                         int32_t n_ops, int32_t out_location, bl_column* outs);
 
+/* ---- rank  (expr.rank(method, descending, seed), plain or .over(partition_by, order_by); polars-ops/src/series/ops/rank.rs) ---- */
+enum { BL_RANK_AVERAGE = 0, BL_RANK_MIN = 1, BL_RANK_MAX = 2, BL_RANK_DENSE = 3, BL_RANK_ORDINAL = 4, BL_RANK_RANDOM = 5 };
+typedef struct bl_rank_op {
+    int32_t method;             /* BL_RANK_* */
+    int32_t descending;         /* rank the largest value 1 */
+    uint64_t seed;              /* BL_RANK_RANDOM */
+    const bl_sort_key* values;  /* a numeric / Boolean column (one chunk) or a LargeUtf8 / LargeBinary column; flags 0 */
+} bl_rank_op;
+/* outs[i] has one row per input row, in input row order.  partition_by / order_by: exactly bl_over's meaning and checks; each
+ * partition is ranked on its own, as rank(...).over(g) is.  The C ABI takes the method explicitly (the Rust default is
+ * Dense, rank.rs:32-39; the Python default is "average").
+ * Per partition (rank.rs:61-188): the non-null values are stably arg-sorted with nulls last and `descending` as given
+ * (:101-107), then split into tie runs where consecutive values are not equal (:117-123), equality being tot_eq: NaN ==
+ * NaN, -0.0 == +0.0 (polars-utils/src/total_ord.rs:321-326).  NaN is the greatest value: last ascending, first descending.
+ * Strings and binary compare their bytes unsigned, a proper prefix first.  A row at sorted position p (0-based among its
+ * partition's non-null rows) in the run [s, e):
+ *   BL_RANK_AVERAGE  Float64, 0.5 ((s + 1) + e) (:141-152), exact for every u32 rank
+ *   BL_RANK_MIN      UInt32, s + 1 (:153-161)
+ *   BL_RANK_MAX      UInt32, e (:162-170)
+ *   BL_RANK_DENSE    UInt32, 1 + the number of runs before this one in the partition (:171-179)
+ *   BL_RANK_ORDINAL  UInt32, p + 1 (:109-116): ties keep the stable order, row order, or with order_by the partition's
+ *                    order_by order (its flags), then row order
+ *   BL_RANK_RANDOM   UInt32, s + 1 + the row's place in a seeded random permutation of its run (:128-140)
+ * A null value gives a null rank (the output validity is the input validity; the null slots hold 0, as the reference's
+ * buffers do); an all-null partition is all null; an empty column gives an empty column of the method's dtype.
+ * Temporal columns: pass their physical Int64.
+ * Not reproduced: BL_RANK_RANDOM.  The reference shuffles each run with one sequential SmallRng, so how many values a run
+ * consumes depends on every earlier run, and no parallel order gives its bytes (its seed-1 answer [2, 5, 7, 3, 4, 6, 1],
+ * py-polars/tests/unit/operations/test_rank.py:27-32, is not this call's).  This call breaks ties by the 32-bit key
+ * fmix32(fmix32(row ^ seed_lo) + seed_hi) (murmur3's finaliser, a bijection of the row index), then takes the ordinal rank:
+ * the ranks of a run are a permutation of [s + 1, e], the same inputs and seed give the same bytes, and the permutation
+ * passes a chi-square test of uniformity.  order_by changes only BL_RANK_ORDINAL.
+ * Exactness: every other method is bit-identical to the reference.
+ * Plan (DESIGN.md §15), per op: bl_arg_sort's stable radix sort of (partition id, value, tie key), then three passes over
+ * the sorted positions: k_rank_heads (tie runs and partition starts as bitmaps, from one gather of the value per position),
+ * k_rank_starts (each run's first position, MIN / MAX / AVERAGE and partitioned ranks only) and k_rank_out (the rank,
+ * scattered to its row).  A string DENSE rank without partitions is bl_string_rank.  Several ops in one call share the
+ * partition ids and the imported keys.
+ * Device memory, beyond the inputs and outputs: the sort's 24 bytes per row (UInt32 permutation, its alternate and two u64
+ * key buffers), up to three position bitmaps (3 / 8 bytes per row), 4 bytes per row of run starts, 4 bytes per row of
+ * RANDOM's tie key and, with partitions, 4 bytes per row of partition ids and 4 to 8 bytes per row of partition starts.
+ * Errors: BL_ERR_INVALID for an unknown method, values->flags != 0, a missing value column, a descriptor with both or neither
+ * of `column` and `strings` set, columns of different lengths and bl_over's key errors; BL_ERR_UNSUPPORTED for Bool
+ * partition columns, more than 2^31 - 1 rows with partitions or order_by and more than 2^32 - 1 rows otherwise. */
+bl_status bl_rank(const bl_sort_key* partition_by, int32_t n_partition_by, const bl_sort_key* order_by, const bl_rank_op* ops, int32_t n_ops,
+                  int32_t out_location, bl_column* outs);
+
 /* ---- K6: radix hash partition (multi-GPU exchange step) --------------------------------- */
 /* partition id = hash_to_partition(dirty_hash(key), n_partitions)
  *              = ((key * 0x55fbfd6bfc5458e9 mod 2^64) * n_partitions) >> 64   (hashing.rs:62-69,132-142),

@@ -1033,6 +1033,73 @@ def rolling_agg(kind: str, column, window_size: int, min_samples=None, center: b
     return rolling([(kind, column, opts)], location=location)[0]
 
 
+RANK_METHODS = {"average": 0, "min": 1, "max": 2, "dense": 3, "ordinal": 4, "random": 5}
+
+
+class BlRankOp(C.Structure):
+    _fields_ = [("method", C.c_int32), ("descending", C.c_int32), ("seed", C.c_uint64), ("values", C.POINTER(BlSortKey))]
+
+
+def _rank_op(column, options: dict, keep: list) -> BlRankOp:
+    """one (column, options) tuple of rank() -> a bl_rank_op"""
+    options = dict(options or {})
+    unknown = set(options) - {"method", "descending", "seed"}
+    if unknown:
+        raise ValueError(f"rank takes no option(s) {', '.join(sorted(unknown))}")
+    method = options.get("method", "average")
+    if method not in RANK_METHODS:
+        raise ValueError(f"unknown rank method {method!r} (one of {', '.join(RANK_METHODS)})")
+    seed = options.get("seed")
+    if seed is None:
+        seed = int.from_bytes(os.urandom(8), "little")
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < 2**64:
+        raise ValueError(f"rank: seed must be an integer in 0..2^64 - 1 or None, not {seed!r}")
+    if column is None:
+        raise ValueError("rank needs a value column")
+    key = C.pointer(_by_key(column, keep))
+    keep.append(key)
+    return BlRankOp(RANK_METHODS[method], int(bool(options.get("descending", False))), int(seed), key)
+
+
+def rank(ops: Sequence, partition_by=(), order_by=None, descending: bool = False, nulls_last: bool = False, location: int = HOST):
+    """bl_rank: `expr.rank(method, descending, seed)`, and with partition_by / order_by `expr.rank(...).over(partition_by,
+    order_by=...)`, one output row per input row.
+    ops: (column, options) tuples; the column is numeric, Bool or a string column (StringColumn / DeviceStringColumn / list
+    of chunks); options: method (one of RANK_METHODS, default "average" as in Polars), descending (default False), seed
+    (for "random"; None draws one).  partition_by / order_by / descending / nulls_last as over() takes them; order_by
+    changes only "ordinal".  Returns one output per op (Float64 for "average", UInt32 otherwise), as gather returns them."""
+    if isinstance(partition_by, (np.ndarray, Column, OutColumn, StringColumn, DeviceStringColumn)):
+        partition_by = [partition_by]
+    partition_by = list(partition_by or [])
+    if isinstance(order_by, list):
+        if len(order_by) != 1:
+            raise ValueError(f"rank() takes one order_by column, not {len(order_by)}")
+        order_by = order_by[0]
+    if not ops:
+        raise ValueError("rank() needs at least one operation")
+    keep = []
+    descs = []
+    for op in ops:
+        if not isinstance(op, tuple) or len(op) != 2:
+            raise ValueError(f"a rank() operation is (column, options), not {op!r}")
+        descs.append(_rank_op(op[0], op[1], keep))
+    parr = (BlSortKey * max(len(partition_by), 1))(*[_by_key(k, keep) for k in partition_by])
+    okey = None
+    if order_by is not None:
+        okey = _by_key(order_by, keep)
+        okey.flags = (SORT_DESCENDING if descending else 0) | (SORT_NULLS_LAST if nulls_last else 0)
+    oarr = (BlRankOp * len(descs))(*descs)
+    outs = (BlColumn * len(descs))()
+    _check(lib().bl_rank(parr if partition_by else None, C.c_int32(len(partition_by)), C.byref(okey) if okey is not None else None, oarr,
+                         C.c_int32(len(descs)), C.c_int32(location), outs))
+    return _finish(list(outs), location)
+
+
+def rank_column(column, method: str = "average", descending: bool = False, seed=None, location: int = HOST):
+    """The plain rank() of a column: rank() with no partition."""
+    return rank([(column, {"method": method, "descending": descending, "seed": seed})], location=location)[0]
+
+
 CLOSED = {"right": 0, "left": 1, "both": 2, "none": 3}
 _NS_OF = {"ns": 1, "us": 1_000, "ms": 1_000_000, "s": 1_000_000_000, "m": 60_000_000_000, "h": 3_600_000_000_000}
 _NS_DAY = 86_400_000_000_000

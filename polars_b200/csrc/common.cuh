@@ -210,6 +210,11 @@ std::vector<DevCol> op_rolling(const std::vector<DevCol>& partition_by, const De
 struct RollByOp { int kind = 0; int closed = 0; int64_t window_size = 1, min_samples = 1; int ddof = 1; const DevCol* values = nullptr; };
 void check_rolling_by_op(int kind, int closed, int64_t window_size, int64_t min_samples, int ddof, int reserved, int value_dtype);
 std::vector<DevCol> op_rolling_by(const std::vector<DevCol>& partition_by, const DevCol& by, const std::vector<RollByOp>& ops, int64_t n);
+// rank (rank.cu): values are numeric / Bool columns (a string column arrives as its ascending dense rank)
+struct RankOp { int method = 0; bool descending = false; uint64_t seed = 0; const DevCol* values = nullptr; };
+void check_rank_op(int method);      // BL_ERR_INVALID for an unknown method
+int rank_dtype(int method);
+std::vector<DevCol> op_rank(const std::vector<DevCol>& partition_by, const DevCol* order_key, int order_flags, const std::vector<RankOp>& ops, int64_t n);
 
 struct JoinResult { DevCol left, right; };
 JoinResult op_hash_join(const DevCol& left, const DevCol& right, int how, bool nulls_equal, int maintain_order);

@@ -13,6 +13,7 @@
 // Errors: `ret` is left untouched (private_data == NULL) and the message is kept thread-local.
 #include <cmath>
 #include <cstdlib>
+#include <random>
 #include <string>
 #include <vector>
 
@@ -140,7 +141,7 @@ static void release_inputs(SeriesExport* inputs, size_t n) {
     }
 }
 
-enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER, P_ROLL, P_ROLL_BY };
+enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER, P_ROLL, P_ROLL_BY, P_RANK };
 
 // ---- kwargs ----------------------------------------------------------------------------------------
 // register_plugin_function(kwargs={...}) pickles the dict (py-polars/src/polars/plugins.py:100-115) and the caller hands
@@ -205,7 +206,7 @@ static int join_how_of(int op) { return op; }
 static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, const Kwargs& kw, SeriesExport* ret) {
     std::lock_guard<std::recursive_mutex> lk(ctx().mu);
     PLB_REQUIRE(n >= 1, BL_ERR_INVALID, "plugin: no input series");
-    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER && kind != P_ROLL && kind != P_ROLL_BY) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
+    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER && kind != P_ROLL && kind != P_ROLL_BY && kind != P_RANK) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
     std::vector<std::vector<bl_column>> chunks(n);
     std::vector<DevCol> in;
     for (size_t i = 0; i < n; i++) { int dt; chunks[i] = input_chunks(inputs[i], &dt); in.push_back(import_column(chunks[i].data(), (int)chunks[i].size())); }
@@ -308,6 +309,24 @@ static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, co
             bl_column h; export_column(r, BL_HOST, &h);
             fill_array(array, h);
             fill_schema(schema, name, format_of(r.dtype));
+        } else if (kind == P_RANK) {
+            // inputs: the values, then the partition keys (none: one partition) -> one row per input row (bl_rank).
+            // kwargs: descending (bool), seed (int for bl_rank_random; absent or None: drawn here)
+            RankOp o;
+            o.method = op; o.descending = kw.get("descending", 0) != 0; o.values = &in[0];
+            const double sd = kw.is_none("seed") ? std::nan("") : kw.get("seed", std::nan(""));
+            if (std::isnan(sd)) { std::random_device rd; o.seed = ((uint64_t)rd() << 32) | rd(); }
+            else {
+                // the kwargs carry numbers as doubles: only integers up to 2^53 arrive exactly
+                PLB_REQUIRE(!kw.is_bool("seed") && sd == std::floor(sd) && sd >= 0 && sd <= 9007199254740992.0, BL_ERR_INVALID,
+                            "plugin rank_*: seed must be an integer in 0..2^53");
+                o.seed = (uint64_t)sd;
+            }
+            const std::vector<DevCol> parts(in.begin() + 1, in.end());
+            const DevCol r = op_rank(parts, nullptr, 0, {o}, in[0].len)[0];
+            bl_column h; export_column(r, BL_HOST, &h);
+            fill_array(array, h);
+            fill_schema(schema, name, format_of(r.dtype));
         } else if (kind == P_GROUP) {
             // inputs: key_0 .. key_{k-1}, value (LEN: keys only)  ->  struct {key, key_1, ..., agg}, groups in first-occurrence order
             const bool is_len = op == BL_AGG_LEN;
@@ -401,6 +420,7 @@ static void field_entry(PluginOp kind, int op, const ArrowSchema* fields, size_t
         case P_OVER: fill_schema(out, name, format_of(over_scan_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_ROLL: fill_schema(out, name, format_of(rolling_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_ROLL_BY: fill_schema(out, name, format_of(rolling_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
+        case P_RANK: fill_schema(out, name, format_of(rank_dtype(op))); break;
         case P_FILTER: case P_GATHER: fill_schema(out, name, format_of(dt < 0 ? BL_INT64 : dt)); break;
         case P_GROUP: {
             const size_t nk = op == BL_AGG_LEN ? n : (n > 0 ? n - 1 : 0);
@@ -485,4 +505,10 @@ PLUGIN(rolling_min_by, P_ROLL_BY, BL_ROLLING_MIN)
 PLUGIN(rolling_max_by, P_ROLL_BY, BL_ROLLING_MAX)
 PLUGIN(rolling_var_by, P_ROLL_BY, BL_ROLLING_VAR)
 PLUGIN(rolling_std_by, P_ROLL_BY, BL_ROLLING_STD)
+PLUGIN(rank_average, P_RANK, BL_RANK_AVERAGE)     /* kwargs: descending, seed (random; None: drawn); inputs = values, then partition keys */
+PLUGIN(rank_min, P_RANK, BL_RANK_MIN)
+PLUGIN(rank_max, P_RANK, BL_RANK_MAX)
+PLUGIN(rank_dense, P_RANK, BL_RANK_DENSE)
+PLUGIN(rank_ordinal, P_RANK, BL_RANK_ORDINAL)
+PLUGIN(rank_random, P_RANK, BL_RANK_RANDOM)
 }
