@@ -532,6 +532,66 @@ typedef struct bl_rolling_by_op {
 bl_status bl_rolling_by(const bl_sort_key* partition_by, int32_t n_partition_by, const bl_column* by, const bl_rolling_by_op* ops,
                         int32_t n_ops, int32_t out_location, bl_column* outs);
 
+/* ---- rolling quantile / median  (expr.rolling_quantile(...) / rolling_quantile_by(by, ...), plain or .over()) ---------- */
+typedef struct bl_rolling_quantile_op {
+    double quantile;          /* [0, 1] */
+    int32_t method;           /* BL_QUANTILE_* */
+    int32_t center;           /* 0 / 1 */
+    int64_t window_size;      /* >= 1 */
+    int64_t min_samples;      /* 0 .. window_size */
+    const bl_column* values;  /* one chunk */
+} bl_rolling_quantile_op;
+typedef struct bl_rolling_quantile_by_op {
+    double quantile;          /* [0, 1] */
+    int32_t method;           /* BL_QUANTILE_* */
+    int32_t closed;           /* BL_CLOSED_* */
+    int64_t window_size;      /* P >= 1, in the physical unit of `by` */
+    int64_t min_samples;      /* >= 0 */
+    const bl_column* values;  /* one chunk */
+} bl_rolling_quantile_by_op;
+/* outs[i] has one row per input row, in input row order.  Partitions, order_by, the window of each row (center; by, closed,
+ * P), the `by` dtypes and units, the order of a shuffled or null `by` and the row limits are exactly bl_rolling's and
+ * bl_rolling_by's.  rolling_median(_by) is quantile 0.5 with BL_QUANTILE_LINEAR (polars-plan/src/dsl/mod.rs:1213-1215,
+ * 1258-1260).  What differs:
+ * Dtype: Float32 stays Float32, every other numeric dtype becomes Float64 (to_float, polars-core/src/series/mod.rs:629-634;
+ * rolling_window/dispatch.rs:314-346), and all arithmetic happens in that type: a Float32 column interpolates in f32 (the
+ * group_by quantile interpolates in f64).  Bool: BL_ERR_UNSUPPORTED.  Temporal value columns: pass their physical Int64.
+ * Window order: the window's non-null values sorted by tot_cmp (NaN greatest, -0.0 == +0.0; SortedBuf, rolling/window.rs).
+ * Index, with m the window's non-null count and all index arithmetic in f64 (no_nulls/quantile.rs:55-105,
+ * nulls/quantile.rs:52-106, quantile_filter.rs:610-671):
+ *   NEAREST       round((m - 1) q), half away from zero, clamped to m - 1
+ *   LOWER         floor((m - 1) q)
+ *   HIGHER        ceil((m - 1) q), clamped to m - 1
+ *   EQUIPROBABLE  max(ceil(m q) - 1, 0)
+ *   MIDPOINT      (lo + hi) / 2 in T when floor((m - 1) q) and ceil((m - 1) q) differ, else lo
+ *   LINEAR        T((m - 1) q - floor((m - 1) q)) * (hi - lo) + lo in T when they differ (quantile_filter.rs:559-567), else lo
+ * There is no lo == hi guard: LINEAR between +inf and +inf is NaN (inf - inf), unlike BL_AGG_QUANTILE.  The three reference
+ * paths (no nulls centered, no nulls trailing through quantile_filter, with nulls) give the same index and arithmetic for q
+ * in [0, 1]; only their clamps differ, and no clamp is reached there.
+ * Validity: a window whose non-null count is below max(min_samples, 1) is null (is_valid, rolling/window.rs:179-181;
+ * create_validity; an all-null window gives None, nulls/quantile.rs:58-61).  A time window also is null when it holds fewer
+ * than min_samples rows, nulls included, or its row's `by` is null (rolling_kernels/shared.rs:109-204).  The Python defaults
+ * are min_samples = window_size for fixed windows and 1 for time windows.
+ * Exactness: bit-identical to the reference, except which of tot_eq values (-0.0 / +0.0, NaN payloads) a result takes: the
+ * reference's sorted buffer leaves that open.  Every result is a value of its window or the interpolation of two of them.
+ * bl_set_deterministic changes nothing.  weights are not in the ABI (the reference's weighted path differs and fails on nulls).
+ * Plan (DESIGN.md §16): per value column, a wavelet matrix over the values' stable ranks (bl_arg_sort with nulls last) in
+ * position order, L = max(1, ceil(log2 rows)) levels of 224-bit blocks with an interleaved rank directory (one 32-byte read
+ * per rank query), then one thread per row: two rank queries per level for the k-th smallest of its window, two descents for
+ * MIDPOINT / LINEAR.  The cost does not depend on the window width.  Ops whose `values` point to the same bl_column share one
+ * matrix.  Device memory, beyond inputs and outputs: the sort's 24 bytes per row (freed before the build), 8 bytes per row of
+ * ranks (two u32 orders), 4 or 8 bytes per row of sorted values, L x rows / 7 bytes of levels (rows / 7 more with nulls),
+ * the 8 bytes per row of window bounds of a time window, and bl_over's order (with its inverse) when a sort is needed.
+ * Errors: BL_ERR_INVALID for a quantile outside [0, 1] or NaN (the reference's rolling path has no range check and indexes
+ * past the window: RollingQuantileParams { prob, method } reaches get_agg unchecked, rolling/mod.rs:140-143,
+ * polars-plan/src/dsl/mod.rs:1181-1196), an unknown method, and otherwise
+ * the window, `by` and key errors of bl_rolling / bl_rolling_by; BL_ERR_UNSUPPORTED for a Bool value column, window_size 0
+ * (fixed windows) and the row limits of bl_rolling / bl_rolling_by. */
+bl_status bl_rolling_quantile(const bl_sort_key* partition_by, int32_t n_partition_by, const bl_sort_key* order_by,
+                              const bl_rolling_quantile_op* ops, int32_t n_ops, int32_t out_location, bl_column* outs);
+bl_status bl_rolling_quantile_by(const bl_sort_key* partition_by, int32_t n_partition_by, const bl_column* by,
+                                 const bl_rolling_quantile_by_op* ops, int32_t n_ops, int32_t out_location, bl_column* outs);
+
 /* ---- rank  (expr.rank(method, descending, seed), plain or .over(partition_by, order_by); polars-ops/src/series/ops/rank.rs) ---- */
 enum { BL_RANK_AVERAGE = 0, BL_RANK_MIN = 1, BL_RANK_MAX = 2, BL_RANK_DENSE = 3, BL_RANK_ORDINAL = 4, BL_RANK_RANDOM = 5 };
 typedef struct bl_rank_op {

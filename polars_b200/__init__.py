@@ -1240,6 +1240,143 @@ def rolling_agg_by(kind: str, column, by, window_size, min_samples=None, closed:
     return rolling_by([(kind, column, opts)], by, location=location)[0]
 
 
+class BlRollingQuantileOp(C.Structure):
+    _fields_ = [("quantile", C.c_double), ("method", C.c_int32), ("center", C.c_int32), ("window_size", C.c_int64), ("min_samples", C.c_int64),
+                ("values", C.POINTER(BlColumn))]
+
+
+class BlRollingQuantileByOp(C.Structure):
+    _fields_ = [("quantile", C.c_double), ("method", C.c_int32), ("closed", C.c_int32), ("window_size", C.c_int64), ("min_samples", C.c_int64),
+                ("values", C.POINTER(BlColumn))]
+
+
+def _rolling_quantile_ops(ops: Sequence, who: str, place: str, keep: list) -> list:
+    """(column, options) tuples -> (quantile, method, place option, window_size option, min_samples option, column struct
+    pointer); ops that pass the same column object share one struct, so the library builds that column's matrix once.
+    place: "center" (fixed windows) or "closed" (time windows)."""
+    if not ops:
+        raise ValueError(f"{who}() needs at least one operation")
+    structs = {}
+    out = []
+    for op in ops:
+        if not isinstance(op, tuple) or len(op) != 2:
+            raise ValueError(f"a {who}() operation is (column, options), not {op!r}")
+        column, options = op[0], dict(op[1] or {})
+        unknown = set(options) - {"quantile", "interpolation", "window_size", "min_samples", place}
+        if unknown:
+            raise ValueError(f"{who} takes no option(s) {', '.join(sorted(unknown))}")
+        for name in ("quantile", "window_size"):
+            if name not in options:
+                raise ValueError(f"{who} needs a {name}")
+        q = options["quantile"]
+        if isinstance(q, bool) or not isinstance(q, (int, float, np.integer, np.floating)) or not 0.0 <= float(q) <= 1.0:
+            raise ValueError(f"{who}: quantile must be a number in [0, 1], not {q!r}")
+        method = options.get("interpolation", "nearest")
+        if method not in QUANTILE_METHODS:
+            raise ValueError(f"{who}: unknown interpolation {method!r} (one of {', '.join(QUANTILE_METHODS)})")
+        if column is None:
+            raise ValueError(f"{who} needs a value column")
+        if id(column) not in structs:
+            c = _as_col(column)
+            st = c.struct()
+            keep.append((c, st))
+            structs[id(column)] = C.pointer(st)
+        out.append((float(q), QUANTILE_METHODS[method], options.get(place), options["window_size"], options.get("min_samples"), structs[id(column)]))
+    return out
+
+
+def rolling_quantile(ops: Sequence, partition_by=(), order_by=None, descending: bool = False, nulls_last: bool = False, location: int = HOST):
+    """bl_rolling_quantile: fixed-window rolling quantiles, one output row per input row (`expr.rolling_quantile(...)` /
+    `rolling_median(...)`, and with partition_by / order_by `.over(partition_by, order_by=...)`).
+    ops: (column, options) tuples; options: quantile (required, in [0, 1]), interpolation (one of QUANTILE_METHODS, default
+    "nearest"), window_size (required), min_samples (default window_size), center (default False).  Ops given the same
+    column object share one device structure.  partition_by / order_by / descending / nulls_last as over() takes them.
+    Returns one Float32 (for a Float32 column) or Float64 output per op, as gather returns them."""
+    if isinstance(partition_by, (np.ndarray, Column, OutColumn, StringColumn, DeviceStringColumn)):
+        partition_by = [partition_by]
+    partition_by = list(partition_by or [])
+    if isinstance(order_by, list):
+        if len(order_by) != 1:
+            raise ValueError(f"rolling_quantile() takes one order_by column, not {len(order_by)}")
+        order_by = order_by[0]
+    keep = []
+    descs = []
+    for q, method, center, ws, ms, ptr in _rolling_quantile_ops(ops, "rolling_quantile", "center", keep):
+        ms = ws if ms is None else ms
+        for name, v in (("window_size", ws), ("min_samples", ms)):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+                raise ValueError(f"rolling_quantile: {name} must be an integer, not {v!r}")
+        if ws < 1:
+            raise ValueError(f"rolling_quantile: window_size must be at least 1, not {ws}")
+        if not 0 <= ms <= ws:
+            raise ValueError(f"rolling_quantile: min_samples ({ms}) must be in 0..window_size ({ws})")
+        descs.append(BlRollingQuantileOp(q, method, int(bool(center)), int(ws), int(ms), ptr))
+    parr = (BlSortKey * max(len(partition_by), 1))(*[_by_key(k, keep) for k in partition_by])
+    okey = None
+    if order_by is not None:
+        okey = _by_key(order_by, keep)
+        okey.flags = (SORT_DESCENDING if descending else 0) | (SORT_NULLS_LAST if nulls_last else 0)
+    oarr = (BlRollingQuantileOp * len(descs))(*descs)
+    outs = (BlColumn * len(descs))()
+    _check(lib().bl_rolling_quantile(parr if partition_by else None, C.c_int32(len(partition_by)), C.byref(okey) if okey is not None else None, oarr,
+                                     C.c_int32(len(descs)), C.c_int32(location), outs))
+    return _finish(list(outs), location)
+
+
+def rolling_quantile_by(ops: Sequence, by, partition_by=(), location: int = HOST):
+    """bl_rolling_quantile_by: time-based rolling quantiles, one output row per input row (`expr.rolling_quantile_by(by,
+    ...)` / `rolling_median_by(...)`, and with partition_by `.over(partition_by)`).
+    ops: (column, options) tuples; options: quantile (required), interpolation (default "nearest"), window_size (required:
+    see window_size_in), min_samples (default 1), closed (default "right").  by: as rolling_by() takes it."""
+    if isinstance(partition_by, (np.ndarray, Column, OutColumn, StringColumn, DeviceStringColumn)):
+        partition_by = [partition_by]
+    partition_by = list(partition_by or [])
+    byc, unit = _by_column(by)
+    keep = []
+    descs = []
+    for q, method, closed, ws, ms, ptr in _rolling_quantile_ops(ops, "rolling_quantile_by", "closed", keep):
+        ws = window_size_in(ws, unit)
+        ms = 1 if ms is None else ms
+        if isinstance(ms, bool) or not isinstance(ms, (int, np.integer)) or ms < 0:
+            raise ValueError(f"rolling_quantile_by: min_samples must be a non-negative integer, not {ms!r}")
+        closed = "right" if closed is None else closed
+        if closed not in CLOSED:
+            raise ValueError(f"rolling_quantile_by: closed must be one of {', '.join(CLOSED)}, not {closed!r}")
+        descs.append(BlRollingQuantileByOp(q, method, CLOSED[closed], ws, int(ms), ptr))
+    bc = _as_col(byc)
+    bst = bc.struct()
+    parr = (BlSortKey * max(len(partition_by), 1))(*[_by_key(k, keep) for k in partition_by])
+    oarr = (BlRollingQuantileByOp * len(descs))(*descs)
+    outs = (BlColumn * len(descs))()
+    _check(lib().bl_rolling_quantile_by(parr if partition_by else None, C.c_int32(len(partition_by)), C.byref(bst), oarr, C.c_int32(len(descs)),
+                                        C.c_int32(location), outs))
+    return _finish(list(outs), location)
+
+
+def rolling_quantile_agg(column, quantile: float, interpolation: str = "nearest", window_size: int = 2, min_samples=None, center: bool = False,
+                         location: int = HOST):
+    """The plain rolling_quantile() of a column: rolling_quantile() with no partition."""
+    return rolling_quantile([(column, {"quantile": quantile, "interpolation": interpolation, "window_size": window_size, "min_samples": min_samples,
+                                       "center": center})], location=location)[0]
+
+
+def rolling_median_agg(column, window_size: int, min_samples=None, center: bool = False, location: int = HOST):
+    """The plain rolling_median() of a column: quantile 0.5, "linear" (the reference's definition)."""
+    return rolling_quantile_agg(column, 0.5, "linear", window_size, min_samples, center, location)
+
+
+def rolling_quantile_agg_by(column, by, quantile: float, window_size, interpolation: str = "nearest", min_samples=None, closed: str = "right",
+                            location: int = HOST):
+    """The plain rolling_quantile_by() of a column: rolling_quantile_by() with no partition."""
+    return rolling_quantile_by([(column, {"quantile": quantile, "interpolation": interpolation, "window_size": window_size, "min_samples": min_samples,
+                                          "closed": closed})], by, location=location)[0]
+
+
+def rolling_median_agg_by(column, by, window_size, min_samples=None, closed: str = "right", location: int = HOST):
+    """The plain rolling_median_by() of a column: quantile 0.5, "linear"."""
+    return rolling_quantile_agg_by(column, by, 0.5, window_size, "linear", min_samples, closed, location)
+
+
 def hash_partition(key, payload: Sequence, n_partitions: int, location: int = HOST):
     k = _as_col(key)
     ps = [_as_col(p) for p in payload]

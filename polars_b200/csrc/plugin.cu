@@ -141,7 +141,7 @@ static void release_inputs(SeriesExport* inputs, size_t n) {
     }
 }
 
-enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER, P_ROLL, P_ROLL_BY, P_RANK };
+enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER, P_ROLL, P_ROLL_BY, P_RANK, P_ROLL_Q, P_ROLL_Q_BY };
 
 // ---- kwargs ----------------------------------------------------------------------------------------
 // register_plugin_function(kwargs={...}) pickles the dict (py-polars/src/polars/plugins.py:100-115) and the caller hands
@@ -203,10 +203,43 @@ static Kwargs parse_kwargs(const uint8_t* p, size_t n) {
 
 static int join_how_of(int op) { return op; }
 
+// closed: "right" / "left" / "both" / "none", or its BL_CLOSED_* code (default "right")
+static int closed_kwarg(const Kwargs& kw) {
+    const std::string cs = kw.gets("closed", "");
+    if (!cs.empty()) {
+        const char* names[] = {"right", "left", "both", "none"};      // BL_CLOSED_RIGHT .. BL_CLOSED_NONE
+        int closed = -1;
+        for (int c = 0; c < 4; c++) if (cs == names[c]) closed = c;
+        PLB_REQUIRE(closed >= 0, BL_ERR_INVALID, "plugin rolling_*_by: unknown closed '" + cs + "'");
+        return closed;
+    }
+    const double c = kw.get("closed", BL_CLOSED_RIGHT);
+    PLB_REQUIRE(!kw.is_bool("closed") && c == std::floor(c) && c >= BL_CLOSED_RIGHT && c <= BL_CLOSED_NONE, BL_ERR_INVALID,
+                "plugin rolling_*_by: closed must be 'right', 'left', 'both', 'none' or its code 0..3");
+    return (int)c;
+}
+
+// quantile (float, required) and method (str, default "nearest"), as group_quantile takes them
+static void quantile_kwargs(const Kwargs& kw, const char* who, double& q, int& method) {
+    q = kw.get("quantile", std::nan(""));
+    PLB_REQUIRE(!std::isnan(q), BL_ERR_INVALID, std::string("plugin ") + who + ": the `quantile` kwarg is required");
+    const std::string m = kw.gets("method", "nearest");
+    static const char* names[] = {"nearest", "lower", "higher", "midpoint", "linear", "equiprobable"};
+    method = -1;
+    for (int j = 0; j < 6; j++) if (m == names[j]) method = j;
+    PLB_REQUIRE(method >= 0, BL_ERR_INVALID, std::string("plugin ") + who + ": unknown method '" + m + "'");
+}
+
+// the kwargs carry numbers as doubles: only integers up to 2^53 arrive exactly
+static void require_int_kwargs(std::initializer_list<double> vs, const char* who) {
+    for (double v : vs)
+        PLB_REQUIRE(v == std::floor(v) && std::fabs(v) <= 9007199254740992.0, BL_ERR_INVALID, std::string("plugin ") + who + ": window_size and min_samples must be integers of at most 2^53");
+}
+
 static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, const Kwargs& kw, SeriesExport* ret) {
     std::lock_guard<std::recursive_mutex> lk(ctx().mu);
     PLB_REQUIRE(n >= 1, BL_ERR_INVALID, "plugin: no input series");
-    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER && kind != P_ROLL && kind != P_ROLL_BY && kind != P_RANK) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
+    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER && kind != P_ROLL && kind != P_ROLL_BY && kind != P_RANK && kind != P_ROLL_Q && kind != P_ROLL_Q_BY) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
     std::vector<std::vector<bl_column>> chunks(n);
     std::vector<DevCol> in;
     for (size_t i = 0; i < n; i++) { int dt; chunks[i] = input_chunks(inputs[i], &dt); in.push_back(import_column(chunks[i].data(), (int)chunks[i].size())); }
@@ -283,29 +316,41 @@ static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, co
             const double ws = kw.is_none("window_size") ? std::nan("") : kw.get("window_size", std::nan(""));
             PLB_REQUIRE(!std::isnan(ws), BL_ERR_INVALID, "plugin rolling_*_by: the `window_size` kwarg is required");
             const double ms = kw.is_none("min_samples") ? (op == BL_ROLLING_SUM ? 0 : 1) : kw.get("min_samples", op == BL_ROLLING_SUM ? 0 : 1);
-            // the kwargs carry numbers as doubles: only integers up to 2^53 arrive exactly
-            for (double v : {ws, ms})
-                PLB_REQUIRE(v == std::floor(v) && std::fabs(v) <= 9007199254740992.0, BL_ERR_INVALID, "plugin rolling_*_by: window_size and min_samples must be integers of at most 2^53");
-            // closed: "right" / "left" / "both" / "none", or its BL_CLOSED_* code
-            int closed = BL_CLOSED_RIGHT;
-            const std::string cs = kw.gets("closed", "");
-            if (!cs.empty()) {
-                const char* names[] = {"right", "left", "both", "none"};      // BL_CLOSED_RIGHT .. BL_CLOSED_NONE
-                closed = -1;
-                for (int c = 0; c < 4; c++) if (cs == names[c]) closed = c;
-                PLB_REQUIRE(closed >= 0, BL_ERR_INVALID, "plugin rolling_*_by: unknown closed '" + cs + "'");
-            } else {
-                const double c = kw.get("closed", BL_CLOSED_RIGHT);
-                PLB_REQUIRE(!kw.is_bool("closed") && c == std::floor(c) && c >= BL_CLOSED_RIGHT && c <= BL_CLOSED_NONE, BL_ERR_INVALID,
-                            "plugin rolling_*_by: closed must be 'right', 'left', 'both', 'none' or its code 0..3");
-                closed = (int)c;
-            }
+            require_int_kwargs({ws, ms}, "rolling_*_by");
+            const int closed = closed_kwarg(kw);
             RollByOp o;
             o.kind = op; o.window_size = (int64_t)ws; o.min_samples = (int64_t)ms;
             o.closed = closed; o.ddof = (int)kw.get("ddof", 1); o.values = &in[0];
             check_rolling_by_op(o.kind, o.closed, o.window_size, o.min_samples, o.ddof, 0, in[0].dtype);
             const std::vector<DevCol> parts(in.begin() + 2, in.end());
             const DevCol r = op_rolling_by(parts, in[1], {o}, in[0].len)[0];
+            bl_column h; export_column(r, BL_HOST, &h);
+            fill_array(array, h);
+            fill_schema(schema, name, format_of(r.dtype));
+        } else if (kind == P_ROLL_Q || kind == P_ROLL_Q_BY) {
+            // rolling_quantile / rolling_median (op 1: quantile 0.5, "linear") and their _by forms.  inputs: the values (then
+            // the `by` column for _by), then the partition keys.  kwargs: quantile and method (rolling_quantile*, as
+            // group_quantile takes them), window_size (int, required; _by: in the physical unit of `by`), min_samples (int;
+            // absent or None: window_size, or 1 for _by), center (bool) or closed (as rolling_*_by)
+            const bool by = kind == P_ROLL_Q_BY;
+            const char* who = by ? "rolling_quantile_by" : "rolling_quantile";
+            PLB_REQUIRE(!by || n >= 2, BL_ERR_INVALID, "plugin rolling_quantile_by: expected the values and the `by` column");
+            RollQuantileOp o;
+            if (op == 0) quantile_kwargs(kw, who, o.quantile, o.method);
+            const double ws = kw.is_none("window_size") ? std::nan("") : kw.get("window_size", std::nan(""));
+            PLB_REQUIRE(!std::isnan(ws), BL_ERR_INVALID, std::string("plugin ") + who + ": the `window_size` kwarg is required");
+            const double ms = kw.is_none("min_samples") ? (by ? 1 : ws) : kw.get("min_samples", by ? 1 : ws);
+            require_int_kwargs({ws, ms}, who);
+            o.window_size = (int64_t)ws; o.min_samples = (int64_t)ms; o.values = &in[0];
+            if (by) {
+                o.closed = closed_kwarg(kw);
+                check_rolling_quantile_by_op(o.quantile, o.method, o.closed, o.window_size, o.min_samples, in[0].dtype);
+            } else {
+                o.center = kw.get("center", 0) != 0;
+                check_rolling_quantile_op(o.quantile, o.method, o.center ? 1 : 0, o.window_size, o.min_samples, in[0].dtype);
+            }
+            const std::vector<DevCol> parts(in.begin() + (by ? 2 : 1), in.end());
+            const DevCol r = by ? op_rolling_quantile_by(parts, in[1], {o}, in[0].len)[0] : op_rolling_quantile(parts, nullptr, 0, {o}, in[0].len)[0];
             bl_column h; export_column(r, BL_HOST, &h);
             fill_array(array, h);
             fill_schema(schema, name, format_of(r.dtype));
@@ -421,6 +466,7 @@ static void field_entry(PluginOp kind, int op, const ArrowSchema* fields, size_t
         case P_ROLL: fill_schema(out, name, format_of(rolling_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_ROLL_BY: fill_schema(out, name, format_of(rolling_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_RANK: fill_schema(out, name, format_of(rank_dtype(op))); break;
+        case P_ROLL_Q: case P_ROLL_Q_BY: fill_schema(out, name, format_of(rolling_quantile_dtype(dt < 0 ? BL_INT64 : dt))); break;
         case P_FILTER: case P_GATHER: fill_schema(out, name, format_of(dt < 0 ? BL_INT64 : dt)); break;
         case P_GROUP: {
             const size_t nk = op == BL_AGG_LEN ? n : (n > 0 ? n - 1 : 0);
@@ -505,6 +551,10 @@ PLUGIN(rolling_min_by, P_ROLL_BY, BL_ROLLING_MIN)
 PLUGIN(rolling_max_by, P_ROLL_BY, BL_ROLLING_MAX)
 PLUGIN(rolling_var_by, P_ROLL_BY, BL_ROLLING_VAR)
 PLUGIN(rolling_std_by, P_ROLL_BY, BL_ROLLING_STD)
+PLUGIN(rolling_quantile, P_ROLL_Q, 0)             /* kwargs: quantile, method, window_size, min_samples, center; inputs = values, then partition keys */
+PLUGIN(rolling_median, P_ROLL_Q, 1)               /* quantile 0.5, "linear" */
+PLUGIN(rolling_quantile_by, P_ROLL_Q_BY, 0)       /* kwargs: quantile, method, window_size, min_samples, closed; inputs = values, by, then partition keys */
+PLUGIN(rolling_median_by, P_ROLL_Q_BY, 1)
 PLUGIN(rank_average, P_RANK, BL_RANK_AVERAGE)     /* kwargs: descending, seed (random; None: drawn); inputs = values, then partition keys */
 PLUGIN(rank_min, P_RANK, BL_RANK_MIN)
 PLUGIN(rank_max, P_RANK, BL_RANK_MAX)

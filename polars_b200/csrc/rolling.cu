@@ -26,17 +26,9 @@ namespace plb {
 // The window state of position i; pre / suf hold the positions from `base` on (global memory: 0; a staged tile: its start).
 template <class St>
 __device__ __forceinline__ typename St::S window_state(const RollArgs& a, int64_t i, const typename St::S* pre, const typename St::S* suf, int64_t base) {
-    int64_t lo = 0, hi = a.n;
-    if (a.offsets) {
-        int64_t gl = 0, gh = a.G;      // offsets[gl] <= i < offsets[gh]
-        while (gh - gl > 1) {
-            const int64_t m = (gl + gh) >> 1;
-            if ((int64_t)__ldg(a.offsets + m) <= i) gl = m; else gh = m;
-        }
-        lo = __ldg(a.offsets + gl); hi = __ldg(a.offsets + gl + 1);
-    }
-    const int64_t s = max(i - a.L, lo), l = min(i + a.R, hi) - 1;
-    const int64_t b = l - (int64_t)((uint32_t)l % a.B);
+    int64_t s, e;
+    const int64_t lo = fixed_window(a, i, s, e);
+    const int64_t l = e - 1, b = l - (int64_t)((uint32_t)l % a.B);
     if (s < b) return St::combine(suf[s - base], pre[l - base]);
     return s == max(b, lo) ? pre[l - base] : suf[s - base];
 }

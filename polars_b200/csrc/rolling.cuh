@@ -99,6 +99,30 @@ struct RollArgs {
     int64_t W;      // time-based windows: the largest we[i] - ws[i]
 };
 constexpr uint32_t BY_NULL = 0xFFFFFFFFu;      // ws[i] of a position whose `by` is null: no window, a null output
+
+// The fixed window [s, e) of position i: [i - L, i + R) clipped to its segment, found by binary search in offsets (none:
+// [0, n)).  Returns the segment's first position.
+__device__ __forceinline__ int64_t fixed_window(const RollArgs& a, int64_t i, int64_t& s, int64_t& e) {
+    int64_t lo = 0, hi = a.n;
+    if (a.offsets) {
+        int64_t gl = 0, gh = a.G;      // offsets[gl] <= i < offsets[gh]
+        while (gh - gl > 1) {
+            const int64_t m = (gl + gh) >> 1;
+            if ((int64_t)__ldg(a.offsets + m) <= i) gl = m; else gh = m;
+        }
+        lo = __ldg(a.offsets + gl); hi = __ldg(a.offsets + gl + 1);
+    }
+    s = max(i - a.L, lo); e = min(i + a.R, hi);
+    return lo;
+}
+
+// The positions of a time-based rolling call (rolling_by.cu): the rows when no partition is given and `by` is non-null and
+// ascending, else bl_over's partition order with `by` as the key, nulls last (need_inv: with its inverse).  Checks the `by`
+// column and the row limits; messages start with `who`.
+struct ByOrder { bool need_order = false; OverOrder o; };
+ByOrder rolling_by_order(const char* who, const std::vector<DevCol>& partition_by, const DevCol& by, int64_t n, bool need_inv);
+// Writes each position's window [ws, we) of width P and `closed` (ws = BY_NULL where `by` is null); returns the widest window
+int64_t rolling_by_bounds(const DevCol& by, const ByOrder& bo, int64_t n, int64_t P, int closed, uint32_t* ws, uint32_t* we);
 template <typename Out> __device__ __forceinline__ Out class_value(const SumFltSt::S& s) {      // get_sum (rolling/sum.rs:98-108)
     const uint32_t nf = s.pinf + s.ninf + s.nan;
     if (nf == 0) return (Out)s.s;

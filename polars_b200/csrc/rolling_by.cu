@@ -314,46 +314,59 @@ void check_rolling_by_op(int kind, int closed, int64_t window_size, int64_t min_
     PLB_REQUIRE(value_dtype != BL_BOOL || kind == BL_ROLLING_SUM, BL_ERR_UNSUPPORTED, "rolling_by: a Boolean column takes only rolling_sum on the device");
 }
 
-// ops are checked by the caller (check_rolling_by_op) before any column is uploaded
-std::vector<DevCol> op_rolling_by(const std::vector<DevCol>& partition_by, const DevCol& by, const std::vector<RollByOp>& ops, int64_t n) {
-    for (auto& op : ops) PLB_REQUIRE(op.values && op.values->len == n, BL_ERR_INVALID, "rolling_by: value columns differ in length");
-    for (auto& k : partition_by) PLB_REQUIRE(k.len == n, BL_ERR_INVALID, "rolling_by: partition columns differ in length");
-    PLB_REQUIRE(by.len == n, BL_ERR_INVALID, "rolling_by: the `by` column differs in length");
+ByOrder rolling_by_order(const char* who, const std::vector<DevCol>& partition_by, const DevCol& by, int64_t n, bool need_inv) {
+    const std::string w = who;
+    PLB_REQUIRE(by.len == n, BL_ERR_INVALID, w + ": the `by` column differs in length");
     PLB_REQUIRE(by.dtype == BL_INT32 || by.dtype == BL_INT64 || by.dtype == BL_UINT32 || by.dtype == BL_UINT64, BL_ERR_INVALID,
-                "rolling_by: a `by` column must be Int32, Int64, UInt32 or UInt64 (Date / Datetime: their physical Int64)");
-    PLB_REQUIRE(n <= 0xFFFFFFFFll, BL_ERR_UNSUPPORTED, "rolling_by: more than 2^32 - 1 rows (IdxSize is u32)");
-    std::vector<DevCol> outs;
-    if (n == 0) {
-        for (auto& op : ops) { outs.push_back(make_col(rolling_dtype(op.kind, op.values->dtype), 0, false)); outs.back().null_count = 0; }
-        return outs;
-    }
+                w + ": a `by` column must be Int32, Int64, UInt32 or UInt64 (Date / Datetime: their physical Int64)");
+    PLB_REQUIRE(n <= 0xFFFFFFFFll, BL_ERR_UNSUPPORTED, w + ": more than 2^32 - 1 rows (IdxSize is u32)");
+    ByOrder bo;
+    if (n == 0) return bo;
     DevPtr st = dev_alloc(3 * 8);
     dev_memset(st->p, 0, 3 * 8);
     PLB_LAUNCH("rolling_by_check", k_rollby_check, grid_for(n, 256), 256, 0, by.v(), by.vm(), by.dtype, n, as<unsigned long long>(st));
     unsigned long long stats[3];
     PLB_CUDA(cudaMemcpyAsync(stats, st->p, sizeof stats, cudaMemcpyDeviceToHost, ctx().stream));
     PLB_CUDA(cudaStreamSynchronize(ctx().stream));
-    PLB_REQUIRE(stats[2] == 0, BL_ERR_INVALID, "rolling_by: a UInt64 `by` value >= 2^63 does not fit the Int64 time (the reference fails on it)");
-    const bool need_order = !partition_by.empty() || stats[0] || stats[1];
-    PLB_REQUIRE(!need_order || n <= 0x7FFFFFFFll, BL_ERR_UNSUPPORTED, "rolling_by: more than 2^31 - 1 rows need a sort (group tuples)");
-    OverOrder o;
-    if (need_order) {
-        o.gid = partition_ids(partition_by, n);
-        build_order(o, &by, BL_SORT_NULLS_LAST, false);
+    PLB_REQUIRE(stats[2] == 0, BL_ERR_INVALID, w + ": a UInt64 `by` value >= 2^63 does not fit the Int64 time (the reference fails on it)");
+    bo.need_order = !partition_by.empty() || stats[0] || stats[1];
+    PLB_REQUIRE(!bo.need_order || n <= 0x7FFFFFFFll, BL_ERR_UNSUPPORTED, w + ": more than 2^31 - 1 rows need a sort (group tuples)");
+    if (bo.need_order) {
+        bo.o.gid = partition_ids(partition_by, n);
+        build_order(bo.o, &by, BL_SORT_NULLS_LAST, need_inv);
+    }
+    return bo;
+}
+
+int64_t rolling_by_bounds(const DevCol& by, const ByOrder& bo, int64_t n, int64_t P, int closed, uint32_t* ws, uint32_t* we) {
+    DevPtr st = dev_alloc(8);
+    dev_memset(st->p, 0, 8);
+    const bool o = bo.need_order;
+    BoundsArgs b{by.v(), by.vm(), by.dtype, o ? as<uint32_t>(bo.o.perm.values) : nullptr, o ? as<uint32_t>(bo.o.offsets.values) : nullptr,
+                 o ? bo.o.G : 1, n, P, closed, ws, we, as<unsigned long long>(st)};
+    PLB_LAUNCH("rolling_by_bounds", k_rollby_bounds, grid_for(n, 256), 256, 0, b);
+    return (int64_t)read_scalar(as<unsigned long long>(st));
+}
+
+// ops are checked by the caller (check_rolling_by_op) before any column is uploaded
+std::vector<DevCol> op_rolling_by(const std::vector<DevCol>& partition_by, const DevCol& by, const std::vector<RollByOp>& ops, int64_t n) {
+    for (auto& op : ops) PLB_REQUIRE(op.values && op.values->len == n, BL_ERR_INVALID, "rolling_by: value columns differ in length");
+    for (auto& k : partition_by) PLB_REQUIRE(k.len == n, BL_ERR_INVALID, "rolling_by: partition columns differ in length");
+    const ByOrder bo = rolling_by_order("rolling_by", partition_by, by, n, false);
+    const bool need_order = bo.need_order;
+    const OverOrder& o = bo.o;
+    std::vector<DevCol> outs;
+    if (n == 0) {
+        for (auto& op : ops) { outs.push_back(make_col(rolling_dtype(op.kind, op.values->dtype), 0, false)); outs.back().null_count = 0; }
+        return outs;
     }
     DevPtr ws = dev_alloc((size_t)n * 4), we = dev_alloc((size_t)n * 4);
     std::vector<DevCol> res;
-    unsigned long long W = 0;
+    int64_t W = 0;
     for (size_t k = 0; k < ops.size(); k++) {
         const RollByOp& op = ops[k];
-        BoundsArgs b{by.v(), by.vm(), by.dtype, need_order ? as<uint32_t>(o.perm.values) : nullptr, need_order ? as<uint32_t>(o.offsets.values) : nullptr,
-                     need_order ? o.G : 1, n, op.window_size, op.closed, as<uint32_t>(ws), as<uint32_t>(we), as<unsigned long long>(st)};
-        if (k == 0 || op.window_size != ops[k - 1].window_size || op.closed != ops[k - 1].closed) {
-            dev_memset(st->p, 0, 8);
-            PLB_LAUNCH("rolling_by_bounds", k_rollby_bounds, grid_for(n, 256), 256, 0, b);
-            PLB_CUDA(cudaMemcpyAsync(&W, st->p, 8, cudaMemcpyDeviceToHost, ctx().stream));
-            PLB_CUDA(cudaStreamSynchronize(ctx().stream));
-        }
+        if (k == 0 || op.window_size != ops[k - 1].window_size || op.closed != ops[k - 1].closed)
+            W = rolling_by_bounds(by, bo, n, op.window_size, op.closed, as<uint32_t>(ws), as<uint32_t>(we));
         // the casts of op_rolling: SUM Int8/16 / UInt8/16 -> Int64, MEAN / VAR / STD in f64, MIN / MAX narrowed back
         const DevCol& v = *op.values;
         const bool small = dtype_is_small_int(v.dtype);
@@ -365,7 +378,7 @@ std::vector<DevCol> op_rolling_by(const std::vector<DevCol>& partition_by, const
         a.values = w.v(); a.validity = w.vm(); a.n = n;
         if (need_order) { a.perm = as<uint32_t>(o.perm.values); a.seg = as<uint32_t>(o.seg.values); a.offsets = as<uint32_t>(o.offsets.values); a.G = o.G; }
         else a.G = 1;
-        a.ws = as<uint32_t>(ws); a.we = as<uint32_t>(we); a.W = (int64_t)W;
+        a.ws = as<uint32_t>(ws); a.we = as<uint32_t>(we); a.W = W;
         a.min_samples = op.min_samples; a.ddof = op.ddof;
         a.out = out.values->p; a.out_valid = as<uint32_t>(out.validity);
         const int kind = op.kind;
