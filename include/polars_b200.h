@@ -309,6 +309,20 @@ typedef struct bl_sort_key {
  * or keys of different lengths: BL_ERR_INVALID.  String payload columns are materialised with bl_string_gather on the
  * permutation, numeric ones with bl_gather. */
 bl_status bl_arg_sort_keys(const bl_sort_key* by, int32_t n_by, int64_t limit, int32_t out_location, bl_column* out_idx);
+/* Top-k selection: the first k rows of the stable order of `by` (flags per key as in bl_arg_sort_keys), as UInt32 row
+ * ids in ASCENDING ROW ORDER; min(k, n) of them.  The same key dtypes as bl_arg_sort_keys; a string / binary key costs
+ * its rank (bl_string_rank), which is a sort of its own.  The reference: top_k / bottom_k of a column
+ * (polars-ops/src/chunked_array/top_k.rs:151-229) put non-null values before nulls, pad with nulls when fewer than k are
+ * valid and leave the output order open (select_nth_unstable); top_k_by / bottom_k_by (top_k.rs:231-297) and
+ * DataFrame.top_k / bottom_k (_arg_bottom_k, polars-core/src/chunked_array/ops/sort/arg_bottom_k.rs:33-…) use
+ * descending = !reverse and nulls_last for every column and return the rows sorted, ties in an open order; sort(...,
+ * limit = k) is the (0, k) slice of the stable order (frame/mod.rs:1482-1486).  This call returns the one set that
+ * answers all of them with ties broken by row index; the sorted form is bl_arg_sort / bl_arg_sort_keys with limit = k
+ * (which selects through this plan when k <= n / 8).  Plan (DESIGN.md §17): an MSD radix select, one histogram pass per
+ * varying 8-bit digit of the key.  Device memory: n / 8 B of selection bitmap, n / 8 B of tie bitmap, row-id lists of at most n / 4 B, the
+ * output.  Errors: k < 0, keys of different lengths, a descriptor with both or neither pointer set: BL_ERR_INVALID; a
+ * key dtype bl_arg_sort does not take: BL_ERR_UNSUPPORTED; more than 2^32 - 1 rows: BL_ERR_UNSUPPORTED. */
+bl_status bl_top_k(const bl_sort_key* by, int32_t n_by, int64_t k, int32_t out_location, bl_column* out_idx);
 
 /* ---- asof join  (_join_asof_dispatch polars-ops/src/frame/join/asof/mod.rs:325-394; by keys groups.rs:39-345) ------- */
 enum { BL_ASOF_BACKWARD = 0, BL_ASOF_FORWARD = 1, BL_ASOF_NEAREST = 2 };

@@ -706,24 +706,24 @@ def _has_string_key(by) -> bool:
     return any(_is_string_key(k) for k in by) if isinstance(by, list) else _is_string_key(by)
 
 
-def _arg_sort_keys(by, descending, nulls_last, limit, location):
-    """bl_arg_sort_keys: `by` holds numeric keys and string keys (a StringColumn / DeviceStringColumn, or a list of chunks)"""
+def _sort_key_descs(by, descending, nulls_last):
+    """`by` (numeric keys and string keys: a StringColumn / DeviceStringColumn, or a list of chunks) -> (bl_sort_key array
+    with the flags, the objects it points into)"""
     keys = by if isinstance(by, list) else [by]
     flags = _sort_flags(len(keys), descending, nulls_last)
     descs, keep = (BlSortKey * len(keys))(), []
     for i, k in enumerate(keys):
-        if _is_string_key(k):
-            chunks = k if isinstance(k, list) else [k]
-            arr = _str_array(chunks)
-            keep.append(arr)
-            descs[i] = BlSortKey(None, C.cast(arr, C.POINTER(BlStringColumn)), len(chunks), flags[i])
-        else:
-            c = _as_col(k)
-            st = c.struct()
-            keep.append((c, st))
-            descs[i] = BlSortKey(C.pointer(st), None, 0, flags[i])
+        d = _by_key(k, keep)
+        d.flags = flags[i]
+        descs[i] = d
+    return descs, keep
+
+
+def _arg_sort_keys(by, descending, nulls_last, limit, location):
+    """bl_arg_sort_keys: `by` holds numeric keys and string keys"""
+    descs, keep = _sort_key_descs(by, descending, nulls_last)
     out = BlColumn()
-    _check(lib().bl_arg_sort_keys(descs, C.c_int32(len(keys)), C.c_int64(-1 if limit is None else int(limit)), C.c_int32(location), C.byref(out)))
+    _check(lib().bl_arg_sort_keys(descs, C.c_int32(len(descs)), C.c_int64(-1 if limit is None else int(limit)), C.c_int32(location), C.byref(out)))
     return _finish([out], location)[0]
 
 
@@ -757,6 +757,65 @@ def sort(by, cols: Sequence, descending=False, nulls_last=False, limit: int | No
     _check(lib().bl_sort(karr, C.c_int32(len(ks)), _sort_flags(len(ks), descending, nulls_last), carr, C.c_int32(len(cs)),
                          C.c_int64(-1 if limit is None else int(limit)), C.c_int32(location), outs))
     return _finish(list(outs)[:len(cs)], location)
+
+
+def arg_top_k(by, k: int, descending=False, nulls_last=False, location: int = HOST):
+    """bl_top_k: the first k rows of the stable order arg_sort(by, descending, nulls_last) gives, as UInt32 row ids in
+    ascending ROW order (arg_sort(..., limit=k) is the same rows in sorted order).  `by` as for arg_sort, string keys
+    included.  Host output: a numpy uint32 array; device output: an OutColumn."""
+    if k < 0:
+        raise ValueError(f"`k` must be non-negative, got {k}")
+    descs, keep = _sort_key_descs(by, descending, nulls_last)
+    out = BlColumn()
+    _check(lib().bl_top_k(descs, C.c_int32(len(descs)), C.c_int64(int(k)), C.c_int32(location), C.byref(out)))
+    res = _finish([out], location)[0]
+    return res[0] if location == HOST else res
+
+
+def _select_sorted(cols: Sequence, by, k: int, descending, location: int):
+    """the payload columns at arg_sort(by, descending, nulls_last=True, limit=k): gather, or string_gather for a string
+    column.  Returns a list like `gather` returns (a string column: a list of bytes / None, or a DeviceStringColumn)."""
+    if k < 0:
+        raise ValueError(f"`k` must be non-negative, got {k}")
+    perm = arg_sort(by, descending=descending, nulls_last=True, limit=k, location=DEVICE)
+    nums = [c for c in cols if not _is_string_key(c)]
+    got = iter(gather(nums, perm, check_bounds=False, location=location) if nums else [])
+    return [string_gather(c, perm, location=location) if _is_string_key(c) else next(got) for c in cols]
+
+
+def top_k(col, k: int, location: int = HOST):
+    """Series.top_k: the k largest values of `col`, largest first and nulls last (fewer than k valid values: padded with
+    the nulls), ties in row order.  The result is gather's / string_gather's for that column."""
+    return _select_sorted([col], col, k, True, location)[0]
+
+
+def bottom_k(col, k: int, location: int = HOST):
+    """Series.bottom_k: the k smallest values of `col`, smallest first and nulls last, ties in row order."""
+    return _select_sorted([col], col, k, False, location)[0]
+
+
+def _reverse_flags(by, reverse) -> list:
+    n_by = len(by) if isinstance(by, list) else 1
+    if isinstance(reverse, (bool, np.bool_)):
+        return [bool(reverse)] * n_by
+    reverse = [bool(x) for x in reverse]
+    if len(reverse) != n_by:
+        raise ValueError(f"the length of `reverse` ({len(reverse)}) does not match the length of `by` ({n_by})")
+    return reverse
+
+
+def top_k_by(cols: Sequence, by, k: int, reverse=False, location: int = HOST):
+    """Expr.top_k_by / DataFrame.top_k: the payload columns `cols` at the k rows that sort first by `by` descending (each
+    column ascending where `reverse` says so), nulls last, in that order; ties in row order.  reverse: a bool or one
+    per `by` column.  Payload dtypes: those gather and string_gather take."""
+    rev = _reverse_flags(by, reverse)
+    return _select_sorted(cols, by, k, [not r for r in rev], location)
+
+
+def bottom_k_by(cols: Sequence, by, k: int, reverse=False, location: int = HOST):
+    """Expr.bottom_k_by / DataFrame.bottom_k: as top_k_by with the k rows that sort first ascending (descending where
+    `reverse` says so)."""
+    return _select_sorted(cols, by, k, _reverse_flags(by, reverse), location)
 
 
 ASOF_STRATEGIES = {"backward": 0, "forward": 1, "nearest": 2}

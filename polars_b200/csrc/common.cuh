@@ -181,6 +181,13 @@ void sort_pairs_u32(uint32_t* keys, uint32_t* vals, int64_t n, int key_bits = 32
 // multi-column arg_sort (sort.cu): flags[i] = BL_SORT_* of by[i]; the UInt32 permutation, truncated to limit (< 0: all rows)
 DevCol op_arg_sort(const std::vector<DevCol>& by, const std::vector<int>& flags, int64_t limit);
 void op_sort(const std::vector<DevCol>& by, const std::vector<int>& flags, const std::vector<DevCol>& cols, int64_t limit, std::vector<DevCol>& outs);
+bool sortable_dtype(int dt);      // the key dtypes op_arg_sort and op_top_k take (sort.cu)
+// the first k rows of op_arg_sort's stable order, as ascending UInt32 row ids (top_k.cu)
+DevCol op_top_k(const std::vector<DevCol>& by, const std::vector<int>& flags, int64_t k);
+DevCol op_mask_rows(const uint32_t* mask, int64_t n);      // the ascending row ids of the set bits (filter.cu)
+void mask_first_into(const uint32_t* mask, int64_t n, int64_t count, uint32_t* out);      // out |= the first `count` set bits of mask (filter.cu)
+// bl_sort_key descriptors -> key columns (string keys as their ascending dense rank) and flags; who: the message prefix
+void import_sort_key_list(const bl_sort_key* by, int32_t n_by, const char* who, std::vector<DevCol>& keys, std::vector<int>& flags);
 void iota_u32(uint32_t* p, int64_t n, uint32_t base);
 inline int bits_for(uint64_t max_value) { int b = 1; while (b < 32 && (max_value >> b)) b++; return b; }   // digits the radix sort has to look at
 

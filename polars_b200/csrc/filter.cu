@@ -206,6 +206,78 @@ void op_filter(const std::vector<DevCol>& cols, const DevCol& mask, std::vector<
     }
 }
 
+// a word per thread, a tile of F_TILE rows per CTA: the thread's word of the mask (cut at n) and the number of set bits
+// before it, from the tile's offset in the scan
+__device__ __forceinline__ uint64_t mask_word_rank(const uint32_t* __restrict__ mask, int64_t n, const uint64_t* __restrict__ tile_off, int64_t t, uint32_t& m,
+                                                   uint32_t* s_warp) {
+    const int64_t w = t * F_TILE_WORDS + threadIdx.x, row0 = w * 32;
+    m = 0;
+    if (row0 < n) {
+        m = mask[w];
+        if (row0 + 32 > n) m &= (1u << (n - row0)) - 1u;
+    }
+    const uint32_t c = __popc(m);
+    uint32_t x = c;      // inclusive warp scan, then the warps before this one
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if (lane_id() >= (unsigned)o) x += y; }
+    if (lane_id() == 31) s_warp[threadIdx.x >> 5] = x;
+    __syncthreads();
+    uint64_t at = tile_off[t] + x - c;
+    for (unsigned v = 0; v < (threadIdx.x >> 5); v++) at += s_warp[v];
+    __syncthreads();
+    return at;
+}
+
+// the row ids of the set bits, ascending
+__global__ void __launch_bounds__(F_TILE_WORDS) k_mask_rows(const uint32_t* __restrict__ mask, int64_t n, const uint64_t* __restrict__ tile_off, int64_t ntiles,
+                                                            uint32_t* __restrict__ out) {
+    __shared__ uint32_t s_warp[F_TILE_WORDS / 32];
+    for (int64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        uint32_t m;
+        uint64_t at = mask_word_rank(mask, n, tile_off, t, m, s_warp);
+        const int64_t row0 = (t * F_TILE_WORDS + threadIdx.x) * 32;
+        for (; m; m &= m - 1) out[at++] = (uint32_t)(row0 + __ffs(m) - 1);
+    }
+}
+
+// out |= the set bits of mask whose rank is below count (each word has one writer)
+__global__ void __launch_bounds__(F_TILE_WORDS) k_mask_first(const uint32_t* __restrict__ mask, int64_t n, const uint64_t* __restrict__ tile_off, int64_t ntiles,
+                                                             int64_t count, uint32_t* __restrict__ out) {
+    __shared__ uint32_t s_warp[F_TILE_WORDS / 32];
+    for (int64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        uint32_t m;
+        const uint64_t at = mask_word_rank(mask, n, tile_off, t, m, s_warp);
+        if (!m || at >= (uint64_t)count) continue;
+        for (int64_t room = count - (int64_t)at, c = __popc(m); c > room; c--) m &= ~(1u << (31 - __clz(m)));      // drop the highest bits
+        out[t * F_TILE_WORDS + threadIdx.x] |= m;
+    }
+}
+
+// per-tile popcounts and their scan (K3's prefix offsets); returns the number of set bits
+static uint64_t mask_tile_offsets(const uint32_t* mask, int64_t n, int64_t ntiles, DevPtr& offs) {
+    DevPtr counts = dev_alloc((size_t)ntiles * 4), tot = dev_alloc(8);
+    offs = dev_alloc((size_t)ntiles * 8);
+    PLB_LAUNCH("k3_tile_counts", k_mask_tile_counts, grid_for(ntiles * 128, 128, 16), 128, 0, mask, n, as<uint32_t>(counts), ntiles);
+    exclusive_scan_u32_to_u64(as<uint32_t>(counts), as<uint64_t>(offs), ntiles, as<uint64_t>(tot));
+    return read_scalar(as<uint64_t>(tot));
+}
+
+DevCol op_mask_rows(const uint32_t* mask, int64_t n) {
+    const int64_t ntiles = (n + F_TILE - 1) / F_TILE;
+    if (n == 0) return make_col(BL_UINT32, 0, false);
+    DevPtr offs;
+    DevCol out = make_col(BL_UINT32, (int64_t)mask_tile_offsets(mask, n, ntiles, offs), false);
+    if (out.len) PLB_LAUNCH("mask_rows", k_mask_rows, grid_for(ntiles * F_TILE_WORDS, F_TILE_WORDS, 16), F_TILE_WORDS, 0, mask, n, as<uint64_t>(offs), ntiles, as<uint32_t>(out.values));
+    return out;
+}
+
+void mask_first_into(const uint32_t* mask, int64_t n, int64_t count, uint32_t* out) {
+    const int64_t ntiles = (n + F_TILE - 1) / F_TILE;
+    if (n == 0 || count <= 0) return;
+    DevPtr offs;
+    mask_tile_offsets(mask, n, ntiles, offs);
+    PLB_LAUNCH("mask_first", k_mask_first, grid_for(ntiles * F_TILE_WORDS, F_TILE_WORDS, 16), F_TILE_WORDS, 0, mask, n, as<uint64_t>(offs), ntiles, count, out);
+}
+
 // ---------------------------------------------------------------------------- radix sort
 // Stable ascending LSD radix sort of (key, u32 value) pairs, 8-bit digits, keys u32 or u64.  It serves the internal
 // ordering modes (maintain_order, ascending row lists of duplicate build keys, GroupsIdx: sort_pairs_u32) and the

@@ -141,7 +141,7 @@ static void release_inputs(SeriesExport* inputs, size_t n) {
     }
 }
 
-enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER, P_ROLL, P_ROLL_BY, P_RANK, P_ROLL_Q, P_ROLL_Q_BY };
+enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER, P_ROLL, P_ROLL_BY, P_RANK, P_ROLL_Q, P_ROLL_Q_BY, P_TOP_K };
 
 // ---- kwargs ----------------------------------------------------------------------------------------
 // register_plugin_function(kwargs={...}) pickles the dict (py-polars/src/polars/plugins.py:100-115) and the caller hands
@@ -239,7 +239,7 @@ static void require_int_kwargs(std::initializer_list<double> vs, const char* who
 static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, const Kwargs& kw, SeriesExport* ret) {
     std::lock_guard<std::recursive_mutex> lk(ctx().mu);
     PLB_REQUIRE(n >= 1, BL_ERR_INVALID, "plugin: no input series");
-    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER && kind != P_ROLL && kind != P_ROLL_BY && kind != P_RANK && kind != P_ROLL_Q && kind != P_ROLL_Q_BY) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
+    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER && kind != P_ROLL && kind != P_ROLL_BY && kind != P_RANK && kind != P_ROLL_Q && kind != P_ROLL_Q_BY && kind != P_TOP_K) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
     std::vector<std::vector<bl_column>> chunks(n);
     std::vector<DevCol> in;
     for (size_t i = 0; i < n; i++) { int dt; chunks[i] = input_chunks(inputs[i], &dt); in.push_back(import_column(chunks[i].data(), (int)chunks[i].size())); }
@@ -278,6 +278,23 @@ static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, co
                 }
             }
             DevCol perm = op_arg_sort(in, flags, -1);
+            bl_column h; export_column(perm, BL_HOST, &h);
+            fill_array(array, h);
+            fill_schema(schema, name, format_of(BL_UINT32));
+        } else if (kind == P_TOP_K) {
+            // inputs: the `by` columns -> the UInt32 ids of the first k rows, best first (DataFrame.top_k / bottom_k:
+            // descending = !reverse for top (op 0), reverse for bottom (op 1), nulls last).  kwargs: k (int, required),
+            // reverse (a bool or an int bitmask, bit i = column i)
+            const double kd = kw.is_none("k") ? std::nan("") : kw.get("k", std::nan(""));
+            PLB_REQUIRE(!std::isnan(kd) && !kw.is_bool("k"), BL_ERR_INVALID, "plugin top_k: the `k` kwarg is required");
+            PLB_REQUIRE(kd == std::floor(kd) && kd >= 0 && kd <= 9007199254740992.0, BL_ERR_INVALID, "plugin top_k: k must be an integer >= 0");
+            const int64_t rv = (int64_t)kw.get("reverse", 0);
+            std::vector<int> flags(n, BL_SORT_NULLS_LAST);
+            for (size_t j = 0; j < n; j++) {
+                const bool reverse = kw.is_bool("reverse") ? rv != 0 : j < 63 && ((rv >> j) & 1);
+                if (reverse == (op == 1)) flags[j] |= BL_SORT_DESCENDING;
+            }
+            DevCol perm = op_arg_sort(in, flags, (int64_t)kd);
             bl_column h; export_column(perm, BL_HOST, &h);
             fill_array(array, h);
             fill_schema(schema, name, format_of(BL_UINT32));
@@ -461,7 +478,7 @@ static void field_entry(PluginOp kind, int op, const ArrowSchema* fields, size_t
     switch (kind) {
         case P_ARITH: fill_schema(out, name, format_of((op == BL_OP_TRUE_DIV && dt >= 0 && dt <= BL_UINT64) ? BL_FLOAT64 : (dt < 0 ? BL_INT64 : dt))); break;
         case P_CMP: fill_schema(out, name, "b"); break;
-        case P_SORT: fill_schema(out, name, format_of(BL_UINT32)); break;
+        case P_SORT: case P_TOP_K: fill_schema(out, name, format_of(BL_UINT32)); break;
         case P_OVER: fill_schema(out, name, format_of(over_scan_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_ROLL: fill_schema(out, name, format_of(rolling_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_ROLL_BY: fill_schema(out, name, format_of(rolling_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
@@ -533,6 +550,8 @@ PLUGIN(join_full_idx, P_JOIN, BL_JOIN_FULL)
 PLUGIN(join_semi_idx, P_JOIN, BL_JOIN_SEMI)
 PLUGIN(join_anti_idx, P_JOIN, BL_JOIN_ANTI)
 PLUGIN(arg_sort, P_SORT, 0)                     /* kwargs: descending, nulls_last (bool or bitmask); inputs = by columns */
+PLUGIN(top_k_idx, P_TOP_K, 0)                   /* kwargs: k, reverse (bool or bitmask); inputs = by columns */
+PLUGIN(bottom_k_idx, P_TOP_K, 1)
 PLUGIN(cum_sum, P_OVER, BL_CUM_SUM)             /* kwargs: reverse; inputs = values, then partition keys */
 PLUGIN(cum_prod, P_OVER, BL_CUM_PROD)
 PLUGIN(cum_min, P_OVER, BL_CUM_MIN)

@@ -59,7 +59,23 @@ __global__ void __launch_bounds__(256) k_sort_encode(const void* __restrict__ co
 bool radix_sort_pairs_u32(uint32_t* k0, uint32_t* v0, uint32_t* k1, uint32_t* v1, int64_t n, uint64_t vary, int* passes_run);
 bool radix_sort_pairs_u64(uint64_t* k0, uint32_t* v0, uint64_t* k1, uint32_t* v1, int64_t n, uint64_t vary, int* passes_run);
 
-static bool sortable_dtype(int dt) { return (dt >= BL_INT8 && dt <= BL_FLOAT64) || dt == BL_BOOL; }
+bool sortable_dtype(int dt) { return (dt >= BL_INT8 && dt <= BL_FLOAT64) || dt == BL_BOOL; }
+
+// limit <= n / SORT_SELECT_DIV takes the selection plan: op_top_k, a gather of the keys at the selected rows, the stable
+// sort of those rows and a gather of the row ids (DESIGN.md §17 measures both sides).  Only for keys the K4 gather moves
+// (4- and 8-byte dtypes); 1- / 2-byte and Bool keys keep the full sort.
+constexpr int64_t SORT_SELECT_DIV = 8;
+// a measurement knob (read per call, as BL_QUANTILE_GLOBAL is): BL_SORT_SELECT_DIV = d selects for limit <= n / d, 0 never
+static bool select_for_limit(int64_t limit, int64_t n) {
+    const char* e = getenv("BL_SORT_SELECT_DIV");
+    const long d = e ? atol(e) : SORT_SELECT_DIV;
+    return limit >= 0 && d >= 1 && limit <= n / d;
+}
+static bool selection_gathers(const std::vector<DevCol>& by) {
+    for (auto& c : by)
+        if (dtype_size(c.dtype) != 4 && dtype_size(c.dtype) != 8) return false;
+    return true;
+}
 
 DevCol op_arg_sort(const std::vector<DevCol>& by, const std::vector<int>& flags, int64_t limit) {
     PLB_REQUIRE(!by.empty(), BL_ERR_INVALID, "arg_sort: no key column");
@@ -70,6 +86,17 @@ DevCol op_arg_sort(const std::vector<DevCol>& by, const std::vector<int>& flags,
         PLB_REQUIRE(sortable_dtype(c.dtype), BL_ERR_UNSUPPORTED, std::string("arg_sort: key dtype ") + dtype_name(c.dtype) + " is not supported");
     }
     PLB_REQUIRE(n <= (int64_t)0xFFFFFFFFll, BL_ERR_UNSUPPORTED, "arg_sort: more than 2^32 - 1 rows (IdxSize is u32)");
+    if (select_for_limit(limit, n) && selection_gathers(by)) {
+        // the selected rows ascend and keep their keys' encoding, so the stable sort of them is the stable order's first
+        // `limit` rows: the same bytes as the full sort below
+        const DevCol ids = op_top_k(by, flags, limit);
+        std::vector<DevCol> sub, composed;
+        if (ids.len) op_gather(by, ids, false, sub);
+        if (sub.empty()) return ids;
+        const DevCol perm = op_arg_sort(sub, flags, -1);
+        op_gather({ids}, perm, false, composed);
+        return composed[0];
+    }
     DevCol out;
     out.dtype = BL_UINT32; out.null_count = 0;
     out.len = limit < 0 ? n : std::min<int64_t>(limit, n);

@@ -262,6 +262,30 @@ DevCol op_string_rank(const DevStr& s, bool descending, int64_t* n_distinct) {
     return out;
 }
 
+void import_sort_key_list(const bl_sort_key* by, int32_t n_by, const char* who, std::vector<DevCol>& keys, std::vector<int>& fl) {
+    const std::string w(who);
+    PLB_REQUIRE(by != nullptr && n_by >= 1, BL_ERR_INVALID, w + ": no key column");
+    int64_t n0 = -1;
+    for (int i = 0; i < n_by; i++) {
+        const bl_sort_key& k = by[i];
+        PLB_REQUIRE((k.column != nullptr) != (k.strings != nullptr), BL_ERR_INVALID,
+                    w + ": key " + std::to_string(i) + " must set exactly one of `column` and `strings`");
+        int64_t len = 0;
+        if (k.column) len = k.column->length;
+        else {
+            PLB_REQUIRE(k.n_chunks >= 1, BL_ERR_INVALID, w + ": string key " + std::to_string(i) + " has no chunks");
+            for (int j = 0; j < k.n_chunks; j++) len += k.strings[j].length;
+        }
+        if (n0 < 0) n0 = len;
+        PLB_REQUIRE(len == n0, BL_ERR_INVALID, w + ": key columns differ in length (" + std::to_string(len) + " != " + std::to_string(n0) + ")");
+    }
+    PLB_REQUIRE(n0 <= (int64_t)0xFFFFFFFFll, BL_ERR_UNSUPPORTED, w + ": more than 2^32 - 1 rows (IdxSize is u32)");      // before any column is read
+    for (int i = 0; i < n_by; i++) {
+        keys.push_back(by[i].column ? import_column(by[i].column, 1) : op_string_rank(import_string(by[i].strings, by[i].n_chunks), false, nullptr));
+        fl.push_back(by[i].flags);
+    }
+}
+
 }  // namespace plb
 
 // ================================================================================ C ABI
@@ -282,26 +306,8 @@ bl_status bl_string_rank(const bl_string_column* chunks, int32_t n_chunks, int32
 bl_status bl_arg_sort_keys(const bl_sort_key* by, int32_t n_by, int64_t limit, int32_t out_location, bl_column* out_idx) {
     BL_TRY
     PLB_REQUIRE(out_idx != nullptr, BL_ERR_INVALID, "arg_sort_keys: null output");
-    PLB_REQUIRE(by != nullptr && n_by >= 1, BL_ERR_INVALID, "arg_sort_keys: no key column");
-    int64_t n0 = -1;
-    for (int i = 0; i < n_by; i++) {
-        const bl_sort_key& k = by[i];
-        PLB_REQUIRE((k.column != nullptr) != (k.strings != nullptr), BL_ERR_INVALID,
-                    "arg_sort_keys: key " + std::to_string(i) + " must set exactly one of `column` and `strings`");
-        int64_t len = 0;
-        if (k.column) len = k.column->length;
-        else {
-            PLB_REQUIRE(k.n_chunks >= 1, BL_ERR_INVALID, "arg_sort_keys: string key " + std::to_string(i) + " has no chunks");
-            for (int j = 0; j < k.n_chunks; j++) len += k.strings[j].length;
-        }
-        if (n0 < 0) n0 = len;
-        PLB_REQUIRE(len == n0, BL_ERR_INVALID, "arg_sort_keys: key columns differ in length (" + std::to_string(len) + " != " + std::to_string(n0) + ")");
-    }
     std::vector<DevCol> keys; std::vector<int> fl;
-    for (int i = 0; i < n_by; i++) {
-        keys.push_back(by[i].column ? import_column(by[i].column, 1) : op_string_rank(import_string(by[i].strings, by[i].n_chunks), false, nullptr));
-        fl.push_back(by[i].flags);
-    }
+    import_sort_key_list(by, n_by, "arg_sort_keys", keys, fl);
     DevCol perm = op_arg_sort(keys, fl, limit);
     export_column(perm, out_location, out_idx);
     BL_CATCH
