@@ -460,17 +460,34 @@ __global__ void k_gb_init(uint64_t* entries, int64_t n_entries, int stride, int 
 // (collision rate of neighbouring rows: skew / sortedness); stats[1], stats[2] are filled by
 // k_gb_estimate_stats (keys seen exactly once / exactly twice in the sample; pairs = sum of c (c - 1) over the sampled
 // multiplicities c, 64-bit: one key on all 65,536 sampled rows gives 4.3e9).
+// The same pass takes the ranges that K5r's packed records need (groupby_radix.cu): of the non-GB_EMPTY keys and of up
+// to GB_SAMPLE_VCOLS 8-byte integer value columns, as order-preserving unsigned patterns (signed: sign bit flipped), with
+// the minima complemented so that the zeroed words are the identity of every update (atomicMax).
 constexpr int GB_CAND_MAX = 1024;
-struct GbSampleStats { unsigned distinct, f1, f2, adjacent, nulls, empties, n_cand, pad; unsigned long long pairs; };
+constexpr int GB_SAMPLE_VCOLS = 4;
+struct GbSampleCols { const uint64_t* v[GB_SAMPLE_VCOLS]; uint64_t flip[GB_SAMPLE_VCOLS]; int32_t n; int32_t pad; uint64_t key_flip; };
+struct GbSampleStats { unsigned distinct, f1, f2, adjacent, nulls, empties, n_cand, pad; unsigned long long pairs;
+                       unsigned long long key_nmin, key_max, v_nmin[GB_SAMPLE_VCOLS], v_max[GB_SAMPLE_VCOLS]; };
 struct GbCandidate { uint64_t key; uint64_t mult; };
-__global__ void k_gb_estimate(const void* keys, const uint32_t* key_validity, int key_dtype, int64_t n, int64_t m, uint64_t* scratch, unsigned* mult, uint64_t cap, int shift, GbSampleStats* stats) {
+__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long x) {
+    for (int o = 16; o > 0; o >>= 1) x = max(x, (unsigned long long)__shfl_xor_sync(0xffffffffu, x, o));
+    return x;
+}
+__global__ void k_gb_estimate(const void* keys, const uint32_t* key_validity, int key_dtype, int64_t n, int64_t m, uint64_t* scratch, unsigned* mult, uint64_t cap, int shift, GbSampleStats* stats,
+                              const __grid_constant__ GbSampleCols C) {
+    unsigned long long knmin = 0, kmax = 0, vnmin[GB_SAMPLE_VCOLS] = {}, vmax[GB_SAMPLE_VCOLS] = {};
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) {
         int64_t row = (int64_t)(((unsigned __int128)i * (unsigned __int128)n) / (unsigned __int128)m);
         bool ins = false, adj = false, isnull = false, isempty = false;
+#pragma unroll
+        for (int c = 0; c < GB_SAMPLE_VCOLS; c++)
+            if (c < C.n) { const unsigned long long o = C.v[c][row] ^ C.flip[c]; vnmin[c] = max(vnmin[c], ~o); vmax[c] = max(vmax[c], o); }
         if (key_validity == nullptr || bit_get(key_validity, row)) {
             uint64_t key = load_key_rt(keys, key_dtype, row);
             adj = row + 1 < n && load_key_rt(keys, key_dtype, row + 1) == key && (key_validity == nullptr || bit_get(key_validity, row + 1));
             if (key != GB_EMPTY) {
+                const unsigned long long o = key ^ C.key_flip;
+                knmin = max(knmin, ~o); kmax = max(kmax, o);
                 uint64_t slot = table_hash(key) >> shift;
                 for (int pr = 0; pr < (int)cap; pr++) {
                     uint64_t k = __ldcg(reinterpret_cast<const unsigned long long*>(scratch + slot));
@@ -494,6 +511,14 @@ __global__ void k_gb_estimate(const void* keys, const uint32_t* key_validity, in
             if (bn) atomicAdd(&stats->nulls, (unsigned)__popc(bn));
             if (be) atomicAdd(&stats->empties, (unsigned)__popc(be));
         }
+    }
+    knmin = warp_max_u64(knmin); kmax = warp_max_u64(kmax);
+#pragma unroll
+    for (int c = 0; c < GB_SAMPLE_VCOLS; c++) if (c < C.n) { vnmin[c] = warp_max_u64(vnmin[c]); vmax[c] = warp_max_u64(vmax[c]); }
+    if (lane_id() == 0) {
+        if (knmin) atomicMax(&stats->key_nmin, knmin);
+        if (kmax) atomicMax(&stats->key_max, kmax);
+        for (int c = 0; c < C.n; c++) { if (vnmin[c]) atomicMax(&stats->v_nmin[c], vnmin[c]); if (vmax[c]) atomicMax(&stats->v_max[c], vmax[c]); }
     }
 }
 // f1 / f2 (keys sampled exactly once / twice), pairs and the heavy-hitter candidates (multiplicity >= hot_thr)
@@ -1020,8 +1045,9 @@ void GroupByState::build_hot_list(const void* cand_v, int n_cand, bool null_hot,
     hot.n_hot = n_hot; hot.null_hot = null_hot ? 1 : 0; hot.empty_hot = empty_hot ? 1 : 0; hot.rows = n_hot + 2;
 }
 
-uint64_t GroupByState::choose_cap(const DevCol& key, int64_t n_total) {
+uint64_t GroupByState::choose_cap(const DevCol& key, int64_t n_total, const std::vector<const DevCol*>* values) {
     double G, G_raw, G_upper = 0, f2 = 0;
+    pack_key = false; pack_cols.clear();
     if (expected_groups > 0) G = G_raw = (double)expected_groups;
     else {
         const int64_t n = key.len, m = std::min<int64_t>(n, 65536);
@@ -1037,7 +1063,16 @@ uint64_t GroupByState::choose_cap(const DevCol& key, int64_t n_total) {
         const unsigned hot_thr = (unsigned)std::max(12.0, std::ceil(hot_rows * (double)m / nt));
         PLB_LAUNCH("k5_fill", k_fill_u64, grid_for(scap, 256), 256, 0, as<uint64_t>(scratch), GB_EMPTY, (int64_t)scap);
         dev_memset(mult->p, 0, scap * 4 + sizeof(GbSampleStats));
-        PLB_LAUNCH("k5_estimate", k_gb_estimate, grid_for(m, 256), 256, 0, key.v(), key.vm(), key.dtype, n, m, as<uint64_t>(scratch), as<unsigned>(mult), scap, 64 - 18, dstats);
+        // value ranges of the distinct 8-byte integer value columns without validity (the columns K5r may pack)
+        GbSampleCols sc; memset(&sc, 0, sizeof sc);
+        sc.key_flip = key.dtype == BL_INT64 ? GB_EMPTY : 0;
+        for (size_t i = 0; values && i < values->size() && i < plans.size(); i++) {
+            const DevCol* v = (*values)[i];
+            if (plans[i].kind == BL_AGG_LEN || !v || v->len != key.len || v->validity || (v->dtype != BL_INT64 && v->dtype != BL_UINT64)) continue;
+            int c = 0; while (c < sc.n && sc.v[c] != v->v()) c++;
+            if (c == sc.n && sc.n < GB_SAMPLE_VCOLS) { sc.v[c] = static_cast<const uint64_t*>(v->v()); sc.flip[c] = v->dtype == BL_INT64 ? GB_EMPTY : 0; sc.n++; }
+        }
+        PLB_LAUNCH("k5_estimate", k_gb_estimate, grid_for(m, 256), 256, 0, key.v(), key.vm(), key.dtype, n, m, as<uint64_t>(scratch), as<unsigned>(mult), scap, 64 - 18, dstats, sc);
         PLB_LAUNCH("k5_estimate", k_gb_estimate_stats, grid_for(scap, 256), 256, 0, as<uint64_t>(scratch), as<unsigned>(mult), (int64_t)scap, hot_thr, dstats, dcand);
         std::vector<unsigned char> hbuf(tail_bytes);
         PLB_CUDA(cudaMemcpyAsync(hbuf.data(), dstats, tail_bytes, cudaMemcpyDeviceToHost, ctx().stream));
@@ -1075,6 +1110,16 @@ uint64_t GroupByState::choose_cap(const DevCol& key, int64_t n_total) {
         // q = m / n of the rows, E[s (s - 1)] = q^2 c (c - 1)
         if (m > 0) { const double q = (double)m / (double)n; f2 = (double)n + (double)st.pairs / (q * q); }
         build_hot_list(cand, (int)std::min<unsigned>(st.n_cand, GB_CAND_MAX), st.nulls >= hot_thr, st.empties >= hot_thr, (double)m);
+        // packed K5r records: a sampled key range at most 2^31 wide gets the window of offsets 0 .. 2^32 - 2 centred on
+        // it (rows outside it are caught by the scatter); value columns within +-2^30 (Int64) / below 2^31 (UInt64)
+        const uint64_t klo = ~st.key_nmin, khi = st.key_max;
+        if (klo <= khi && khi - klo <= (1ull << 31)) { pack_key = true; pack_base = (klo ^ sc.key_flip) + (khi - klo) / 2 - 0x7FFFFFFFull; }
+        for (int c = 0; c < sc.n; c++) {
+            const uint64_t lo = ~st.v_nmin[c] ^ sc.flip[c], hi = st.v_max[c] ^ sc.flip[c];
+            if (~st.v_nmin[c] > st.v_max[c]) continue;
+            const bool fits = sc.flip[c] ? (int64_t)lo >= -(1ll << 30) && (int64_t)hi <= (1ll << 30) : hi < (1ull << 31);
+            if (fits) pack_cols.push_back(sc.v[c]);
+        }
     }
     est_groups = (int64_t)(G_raw * 1.25) + 2;      // for the shared-memory plan (overflow falls through to the global table)
     // floor by Cauchy-Schwarz, F2 >= n^2 / groups: a strided sample of sorted or clustered keys sees a group at most once
@@ -1163,14 +1208,19 @@ static void launch_smem(const GbLayout& L, const GbTableDev& T, const GbBatch& B
 // Per-batch column binding: aggregations over the same buffer share one column slot; col_kbegin / wslot / wop list each
 // column's accumulator words, null counters only where the column carries a validity bitmap.  pw != 0 (pair layout): the
 // column of the paired integer sum is bound first (column 0: the bulk-reduce kernels read it with a static index) and
-// pair_k is set.  false: more than max_cols distinct value columns.
-bool GroupByState::bind_columns(const DevCol& key, const std::vector<const DevCol*>& values, int64_t row_base, int pw, int max_cols, GbBatch& B, GbLayout& Lb) const {
+// pair_k is set.  first_col != nullptr: the column with that buffer is bound first (K5r's packed records carry column 0
+// in the key's word).  false: more than max_cols distinct value columns.
+bool GroupByState::bind_columns(const DevCol& key, const std::vector<const DevCol*>& values, int64_t row_base, int pw, int max_cols, GbBatch& B, GbLayout& Lb,
+                                const void* first_col) const {
     memset(&B, 0, sizeof B);
     B.keys = key.v(); B.key_validity = key.vm(); B.n = key.len; B.row_base = (uint32_t)row_base; B.key_dtype = key.dtype;
     std::vector<const void*> col_ptr; std::vector<int> col_of_agg(plans.size(), -1);
     std::vector<size_t> plan_order;
-    for (size_t i = 0; i < plans.size(); i++) if (pw && plans[i].main == pw - 2) plan_order.push_back(i);
-    for (size_t i = 0; i < plans.size(); i++) if (!(pw && plans[i].main == pw - 2)) plan_order.push_back(i);
+    auto first = [&](size_t i) {
+        return (pw && plans[i].main == pw - 2) || (first_col && plans[i].kind != BL_AGG_LEN && values[i] && values[i]->v() == first_col);
+    };
+    for (size_t i = 0; i < plans.size(); i++) if (first(i)) plan_order.push_back(i);
+    for (size_t i = 0; i < plans.size(); i++) if (!first(i)) plan_order.push_back(i);
     for (size_t i : plan_order) {
         if (plans[i].kind == BL_AGG_LEN) continue;
         const DevCol* v = values[i];
@@ -1324,9 +1374,9 @@ void GroupByState::consume_pipelined(const DevCol& key, const std::vector<const 
 void GroupByState::consume_all(const DevCol& key, const std::vector<const DevCol*>& values) {
     PLB_REQUIRE(key.dtype == key_dtype, BL_ERR_DTYPE, "group_by: key dtype differs from the plan");
     PLB_REQUIRE(key.len <= 0xFFFFFFFEll, BL_ERR_UNSUPPORTED, "group_by: more than 2^32-2 rows (IdxSize = u32)");
-    uint64_t c = choose_cap(key, key.len);
+    uint64_t c = choose_cap(key, key.len, &values);
     note_batch_shape(key, values);
-    if (consume_radix(key, values, c)) return;      // tables beyond L2: partition the rows instead (groupby_radix.cu)
+    if (consume_radix(key, values, c)) return;     // tables beyond L2: partition the rows instead (groupby_radix.cu)
     // optimistic: no host round trip here — finish() reads the status word together with the group count and, if the sampled
     // estimate was too small, redoes the batch into a table 8x larger (the inputs outlive the state in every caller)
     alloc_table(c);

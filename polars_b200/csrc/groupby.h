@@ -96,6 +96,11 @@ struct GroupByState {
     int64_t est_groups = 0;      // sampled / hinted cardinality; selects the shared-memory plan
     double sample_adjacent = 0;  // sampled fraction of rows whose successor carries the same key (skew / sortedness)
     double est_f2 = 0;           // sampled sum over groups of (rows in the group)^2 in the batch (0: not sampled); sizes K5r's bucket streams
+    // sampled ranges for K5r's packed records (choose_cap): the key fits the window of 2^32 - 1 offsets from pack_base,
+    // and the 8-byte integer value columns in pack_cols fit 32 bits (Int64 within +-2^30, UInt64 below 2^31)
+    bool pack_key = false;
+    uint64_t pack_base = 0;
+    std::vector<const void*> pack_cols;
     GbHotDev hot{};              // heavy hitters found in the sample (rows == 0: none)
     double hot_share = 0;        // sampled share of the hottest key
     DevPtr hot_buf;
@@ -124,9 +129,10 @@ struct GroupByState {
    private:
     void alloc_table(uint64_t new_cap);
     int smem_table_cap() const;
-    bool bind_columns(const DevCol& key, const std::vector<const DevCol*>& values, int64_t row_base, int pw, int max_cols, GbBatch& B, GbLayout& Lb) const;
+    bool bind_columns(const DevCol& key, const std::vector<const DevCol*>& values, int64_t row_base, int pw, int max_cols, GbBatch& B, GbLayout& Lb,
+                      const void* first_col = nullptr) const;
     void note_batch_shape(const DevCol& key, const std::vector<const DevCol*>& values);
-    uint64_t choose_cap(const DevCol& key, int64_t n_total);
+    uint64_t choose_cap(const DevCol& key, int64_t n_total, const std::vector<const DevCol*>* values = nullptr);
     void build_hot_list(const void* candidates, int n_cand, bool null_hot, bool empty_hot, double sample_rows);
     void launch_batch(const DevCol& key, const std::vector<const DevCol*>& values, int64_t row_base);
     void grow(uint64_t new_cap);

@@ -7,7 +7,8 @@
 //   pass 0  k_gbr_hist      rows per bucket (bucket = top bits of table_hash(key): the slot function of the L2 plan), only
 //                           when the sample cannot size the bucket streams (consume_radix: "exact" sizing)
 //   pass 1  k_gbr_scatter   every CTA sorts a 2048-row tile by bucket in shared memory as ROW-MAJOR records
-//                           [key, v0, v1, ...] and writes each (tile, bucket) run with ONE cp.async.bulk (TMA)
+//                           [key, v0, v1, ...] (packed: [key offset | v0, v1, ...], see GbRadixDev) and writes each
+//                           (tile, bucket) run with ONE cp.async.bulk (TMA)
 //                           shared->global copy (runs padded to an even record count with a GB_EMPTY-key record so both
 //                           ends stay 16-byte aligned).  Past 512 buckets the runs shrink to single records:
 //           k_gbr_scatter_wc    instead collects every bucket's rows in a 4-record chunk buffer in shared memory
@@ -23,9 +24,13 @@
 // While the L2 plan's table stays in L2 this plan loses to it (64-bit shared-memory atomics on random slots cost several
 // SM cycles per row), so it is only taken when the L2 plan's table would exceed the L2 budget.
 // Restrictions (anything else stays on the L2 plan): no validity bitmaps, no first-row tracking, <= 4 value columns,
-// no heavy hitters in the sample.  Exact for any input: a bucket that outgrows the stream the sample sized for it raises
-// status 2 and the caller redoes the batch with capacities from the exact histogram; a bucket with more groups than its
-// shared-memory table holds raises status 1 and the caller redoes the batch on the L2 plan.
+// no heavy hitters in the sample.  Records are packed (one 8-byte word less) when the sample puts the key in a window of
+// 2^32 - 1 offsets and one value column in 32 bits; the plan (buckets, table, store path, stream sizing) is the one of
+// the plain width either way.  Exact for any input: a row outside the packed form raises status 4 and the caller redoes
+// the batch with plain records; a bucket that outgrows the stream the sample sized for it raises status 2 and the
+// caller redoes the batch with capacities from the exact histogram (both at once: one redo, plain and exactly sized);
+// a bucket with more groups than its shared-memory table holds raises status 1 and the caller redoes the batch on the
+// L2 plan.
 #include <algorithm>
 #include <cstdlib>
 
@@ -39,21 +44,61 @@ namespace plb {
 constexpr int GBR_THREADS = 512;      // pass 1: 2048-row tiles (bulk stores) / 4096-row tiles (many buckets: longer runs per bucket)
 constexpr int GBR_MAX_LOGB = 13;
 constexpr int GBR_NCW = 31, GBR_NCT = GBR_NCW * 32;                                    // pass 2: 31 consumer warps + 1 producer warp
-// pass 1: a reservation that would end past its bucket's stream (R.cap records) stores nothing and sets status 2; pass 2
+// pass 1: a reservation that would end past its bucket's stream (R.cap records) stores nothing and sets status 2 (GBR_ST_STREAM); pass 2
 // then returns at entry and the caller redoes the batch with exact sizing.  The bound is a kernel parameter rather than
 // off[p + 1] - off[p]: two more loads per reservation made ptxas spill in k_gbr_scatter_wc<3, 8, *>.
 constexpr unsigned GBR_NO_ROOM = 0xFFFFFFFFu;
 
+// status bits (atomicOr: one attempt may raise several; pass 2 returns at entry on GBR_ST_STREAM | GBR_ST_UNFIT)
+constexpr int GBR_ST_TABLE = 1;       // a bucket's pass-2 table overflowed (or the dense output bound): the L2 plan redoes the batch
+constexpr int GBR_ST_STREAM = 2;      // a bucket's record stream overflowed (pass 1): redone with exact sizing
+constexpr int GBR_ST_UNFIT = 4;       // a row does not fit the packed records (pass 1): redone with plain records
+
 struct GbRadixDev {
-    uint64_t* recs;                 // record streams, bucket b at recs + off[b] * roww
+    uint64_t* recs;                 // record streams, bucket b at recs + off[b] * (record words)
     const unsigned long long* off;  // first record of bucket b (even; a multiple of GBR_WC_F for the write-combining scatter)
     unsigned* cursor;               // records written to bucket b so far (pads included)
     unsigned* counts;               // pass 0 (exact sizing): rows of bucket b
     int logB, roww;
     uint64_t* special;              // accumulator row of the GB_EMPTY-key group: [len, words...] (RED target; rare rows only)
     unsigned cap;                   // records of every bucket stream (sample sizing); ~0u: exact sizing, whose streams hold their rows by construction
-    int* status;                    // 1: a bucket's pass-2 table overflowed; 2: a bucket's record stream overflowed (pass 1)
+    int* status;                    // GBR_ST_* bits
+    // Packed records (the PACK form of the kernels): word 0 = (key - pk_base) as a u32 in its low half and value column 0
+    // as a u32 in its high half, columns 1.. in their own words: ROWW - 1 words instead of ROWW.  Offset GBR_PK_PAD is the
+    // pad marker.  Column 0 widens back to the 64-bit raw pattern by sign extension (Int64) or zero extension (4-byte
+    // columns, whose raw pattern is the zero-extended value, and UInt64).
+    uint64_t pk_base;
+    int pk_sext;
 };
+constexpr uint32_t GBR_PK_PAD = 0xFFFFFFFFu;
+// word 0 of a packed record; fit = false when the key lies outside the window or the value does not widen back to itself
+__device__ __forceinline__ uint64_t gbr_pack(const GbRadixDev& R, uint64_t key, uint64_t v, bool& fit) {
+    const uint64_t off = key - R.pk_base, wide = R.pk_sext ? (uint64_t)(int64_t)(int32_t)(uint32_t)v : (uint64_t)(uint32_t)v;
+    fit = off < GBR_PK_PAD && wide == v;
+    return (uint64_t)(uint32_t)off | (v << 32);
+}
+__device__ __forceinline__ uint64_t gbr_unpack_value(const GbRadixDev& R, uint64_t w) {
+    return R.pk_sext ? (uint64_t)(int64_t)(int32_t)(uint32_t)(w >> 32) : w >> 32;
+}
+// record words of the unpacked width ROWW
+template <int ROWW, bool PACK> constexpr int gbr_rw() { return PACK ? ROWW - 1 : ROWW; }
+// one record at rec: [key, v0, v1, ...] or, packed, [pack(key, v0), v1, ...].  A row that does not fit the packed form
+// raises GBR_ST_UNFIT (the status is read first: rows of a batch that misses the window would otherwise queue atomics on
+// one address).  Its record is written all the same: pass 2 does not run on such a batch.
+template <int NC, bool PACK, class Val>
+__device__ __forceinline__ void gbr_put(uint64_t* rec, const GbRadixDev& R, uint64_t key, Val val) {
+    if constexpr (PACK) {
+        bool fit;
+        rec[0] = gbr_pack(R, key, val(0), fit);
+        if (!fit && !(*reinterpret_cast<volatile int*>(R.status) & GBR_ST_UNFIT)) atomicOr(R.status, GBR_ST_UNFIT);
+#pragma unroll
+        for (int c = 1; c < NC; c++) rec[c] = val(c);
+    } else {
+        rec[0] = key;
+#pragma unroll
+        for (int c = 0; c < NC; c++) rec[1 + c] = val(c);
+    }
+}
 
 // gb_load_pair of rows r0, r0 + 1 with a bounds check against n (rows past the end read as 0)
 template <int KEY_ELEM> __device__ __forceinline__ void gbr_load_pair(const void* col, int64_t r0, int64_t n, uint64_t& a, uint64_t& b) {
@@ -148,13 +193,13 @@ __device__ __forceinline__ void gbr_apply_special(const GbLayout& L, const GbBat
 }
 
 constexpr int GBR_RPT = 4;      // rows per thread: 2048-row tiles (8 rows per thread, 4096-row tiles at 1 CTA / SM, was slower)
-template <int ROWW, int KEY_ELEM, int KEY_CANON, bool BULK>
+template <int ROWW, int KEY_ELEM, int KEY_CANON, bool BULK, bool PACK>
 __global__ void __launch_bounds__(GBR_THREADS) k_gbr_scatter(const __grid_constant__ GbLayout L, const __grid_constant__ GbBatch Bt, const __grid_constant__ GbRadixDev R) {
-    constexpr int RPT = GBR_RPT, T = GBR_THREADS * RPT, THREADS = GBR_THREADS, NC = ROWW - 1;
+    constexpr int RPT = GBR_RPT, T = GBR_THREADS * RPT, THREADS = GBR_THREADS, NC = ROWW - 1, RW = gbr_rw<ROWW, PACK>();
     const int logB = R.logB, B = 1 << logB;
     extern __shared__ __align__(16) uint64_t gbr_smem[];
     uint64_t* stage = gbr_smem;                                        // (T + (BULK ? B : 0)) records
-    unsigned* hist = reinterpret_cast<unsigned*>(stage + (size_t)(T + (BULK ? B : 0)) * ROWW);
+    unsigned* hist = reinterpret_cast<unsigned*>(stage + (size_t)(T + (BULK ? B : 0)) * RW);
     unsigned* start = hist + B;
     unsigned* gpos = start + B;
     uint16_t* sp = reinterpret_cast<uint16_t*>(gpos + B);             // !BULK: bucket of every sorted slot
@@ -201,16 +246,16 @@ __global__ void __launch_bounds__(GBR_THREADS) k_gbr_scatter(const __grid_consta
                 const unsigned c = hist[p], cp = BULK ? ((c + 1u) & ~1u) : c;
                 start[p] = run;
                 unsigned g = cp ? atomicAdd(&R.cursor[p], cp) : 0u;
-                if (g + cp > R.cap) { *R.status = 2; g = GBR_NO_ROOM; }
+                if (g + cp > R.cap) { atomicOr(R.status, GBR_ST_STREAM); g = GBR_NO_ROOM; }
                 gpos[p] = g;
                 run += cp;
             }
         }
         if (BULK) bulk_wait_read0();        // the previous tile's copies have finished reading the staging buffer
         __syncthreads();
-        if (BULK) for (int p = tid; p < B; p += THREADS) { const unsigned c = hist[p]; if (c & 1u) { uint64_t* pad = stage + (size_t)(start[p] + c) * ROWW; pad[0] = GB_EMPTY;
+        if (BULK) for (int p = tid; p < B; p += THREADS) { const unsigned c = hist[p]; if (c & 1u) { uint64_t* pad = stage + (size_t)(start[p] + c) * RW; pad[0] = PACK ? GBR_PK_PAD : GB_EMPTY;
 #pragma unroll
-                                                                                                      for (int w = 1; w < ROWW; w++) pad[w] = 0; } }
+                                                                                                      for (int w = 1; w < RW; w++) pad[w] = 0; } }
         // place the records (order inside a run is arbitrary)
 #pragma unroll
         for (int j = 0; j < RPT / 2; j++) {
@@ -230,10 +275,7 @@ __global__ void __launch_bounds__(GBR_THREADS) k_gbr_scatter(const __grid_consta
                     continue;
                 }
                 const unsigned bkt = q >> 16, pos = start[bkt] + (q & 0xFFFFu);
-                uint64_t* rec = stage + (size_t)pos * ROWW;
-                rec[0] = k[2 * j + e];
-#pragma unroll
-                for (int c = 0; c < NC; c++) rec[1 + c] = v[c][e];
+                gbr_put<NC, PACK>(stage + (size_t)pos * RW, R, k[2 * j + e], [&](int c) { return v[c][e]; });
                 if (!BULK) sp[pos] = (uint16_t)bkt;
             }
         }
@@ -242,15 +284,15 @@ __global__ void __launch_bounds__(GBR_THREADS) k_gbr_scatter(const __grid_consta
         if (BULK) {
             for (int p = tid; p < B; p += THREADS) {
                 const unsigned c = hist[p], cp = (c + 1u) & ~1u;
-                if (cp && gpos[p] != GBR_NO_ROOM) bulk_s2g(R.recs + (R.off[p] + gpos[p]) * ROWW, stage + (size_t)start[p] * ROWW, cp * ROWW * 8);
+                if (cp && gpos[p] != GBR_NO_ROOM) bulk_s2g(R.recs + (R.off[p] + gpos[p]) * RW, stage + (size_t)start[p] * RW, cp * RW * 8);
             }
             bulk_commit();
         } else {
             const unsigned total = start[B - 1] + hist[B - 1];
-            for (unsigned w = tid; w < total * ROWW; w += THREADS) {
-                const unsigned row = w / ROWW, c = w - row * ROWW;
+            for (unsigned w = tid; w < total * RW; w += THREADS) {
+                const unsigned row = w / RW, c = w - row * RW;
                 const unsigned p = sp[row], g = gpos[p];
-                if (g != GBR_NO_ROOM) R.recs[(R.off[p] + g + (row - start[p])) * ROWW + c] = stage[w];
+                if (g != GBR_NO_ROOM) R.recs[(R.off[p] + g + (row - start[p])) * RW + c] = stage[w];
             }
             __syncthreads();
         }
@@ -278,9 +320,10 @@ __device__ __forceinline__ void gbr_wc_load(const GbBatch& Bt, int64_t base, uin
     }
 }
 
-template <int ROWW, int KEY_ELEM, int KEY_CANON>
+template <int ROWW, int KEY_ELEM, int KEY_CANON, bool PACK>
 __global__ void __launch_bounds__(GBR_WC_THREADS, 2) k_gbr_scatter_wc(const __grid_constant__ GbLayout L, const __grid_constant__ GbBatch Bt, const __grid_constant__ GbRadixDev R) {
-    constexpr int THREADS = GBR_WC_THREADS, F = GBR_WC_F, RPT = gbr_wc_rpt<ROWW>(), T = THREADS * RPT, NC = ROWW - 1, NCX = NC > 0 ? NC : 1, CH = F * ROWW;
+    constexpr int THREADS = GBR_WC_THREADS, F = GBR_WC_F, RPT = gbr_wc_rpt<ROWW>(), T = THREADS * RPT, NC = ROWW - 1, NCX = NC > 0 ? NC : 1, RW = gbr_rw<ROWW, PACK>(),
+                  CH = F * RW;
     constexpr unsigned NONE = 0xFFFFFFFFu;
     const int logB = R.logB, B = 1 << logB, tid = threadIdx.x;
     extern __shared__ __align__(16) uint64_t gbr_smem[];
@@ -324,10 +367,7 @@ __global__ void __launch_bounds__(GBR_WC_THREADS, 2) k_gbr_scatter_wc(const __gr
             for (int e = 0; e < RPT; e++) {
                 const unsigned s = pk[e] & 0xFFFFu;
                 if (pk[e] == NONE || s / F != r) continue;
-                uint64_t* rec = buf + (size_t)(pk[e] >> 16) * CH + (s % F) * ROWW;
-                rec[0] = k[e];
-#pragma unroll
-                for (int c = 0; c < NC; c++) rec[1 + c] = v[c][e];
+                gbr_put<NC, PACK>(buf + (size_t)(pk[e] >> 16) * CH + (s % F) * RW, R, k[e], [&](int c) { return v[c][e]; });
             }
             fence_async_smem();
             const bool more = __syncthreads_or(last > r);
@@ -349,8 +389,8 @@ __global__ void __launch_bounds__(GBR_WC_THREADS, 2) k_gbr_scatter_wc(const __gr
                 for (int q = 0; q < 4; q++) {
                     const int p = p0 + q * THREADS + tid;
                     if (g[q] == NONE) continue;
-                    if (g[q] + F <= R.cap) bulk_s2g(R.recs + (R.off[p] + g[q]) * ROWW, buf + (size_t)p * CH, CH * 8);
-                    else *R.status = 2;
+                    if (g[q] + F <= R.cap) bulk_s2g(R.recs + (R.off[p] + g[q]) * RW, buf + (size_t)p * CH, CH * 8);
+                    else atomicOr(R.status, GBR_ST_STREAM);
                 }
             }
             bulk_commit();
@@ -359,17 +399,17 @@ __global__ void __launch_bounds__(GBR_WC_THREADS, 2) k_gbr_scatter_wc(const __gr
             __syncthreads();
         }
     }
-    // partial chunks, padded to F records with GB_EMPTY keys (their buffers are not in flight: a chunk that left in the
-    // last round was full, which leaves its bucket's buffer empty)
+    // partial chunks, padded to F records with GB_EMPTY keys / GBR_PK_PAD offsets (their buffers are not in flight: a
+    // chunk that left in the last round was full, which leaves its bucket's buffer empty)
     __syncthreads();
     for (int p = tid; p < B; p += THREADS) {
         const unsigned f = fill[p];
         if (f == 0) continue;
-        for (unsigned i = f; i < F; i++) buf[(size_t)p * CH + i * ROWW] = GB_EMPTY;
+        for (unsigned i = f; i < F; i++) buf[(size_t)p * CH + i * RW] = PACK ? GBR_PK_PAD : GB_EMPTY;
         fence_async_smem();
         const unsigned g = atomicAdd(&R.cursor[p], (unsigned)F);
-        if (g + F <= R.cap) bulk_s2g(R.recs + (R.off[p] + g) * ROWW, buf + (size_t)p * CH, CH * 8);
-        else *R.status = 2;
+        if (g + F <= R.cap) bulk_s2g(R.recs + (R.off[p] + g) * RW, buf + (size_t)p * CH, CH * 8);
+        else atomicOr(R.status, GBR_ST_STREAM);
     }
     bulk_commit();
     bulk_wait0();
@@ -378,19 +418,22 @@ __global__ void __launch_bounds__(GBR_WC_THREADS, 2) k_gbr_scatter_wc(const __gr
 // ---------------------------------------------------------------------------- pass 2: TMA ring -> shared-memory table -> dense output
 struct GbDenseDev { uint64_t* keys; uint32_t* first; uint32_t* len; uint64_t* words; int64_t Gb; unsigned long long* cursor; };
 
-constexpr int GBR_NST = 2;      // ring stages
-template <int ROWW>
+constexpr int GBR_NST = 2;      // ring stages of plain records
+// the ring keeps the bytes of GBR_NST stages of plain ROWW-word records (the plan's table size S depends on them); packed
+// records fill that room with more stages (3 of 2 words where 2 of 3 were)
+template <int ROWW, bool PACK> constexpr int gbr_nst() { return GBR_NST * ROWW / gbr_rw<ROWW, PACK>(); }
+template <int ROWW, bool PACK>
 __global__ void __launch_bounds__(1024) k_gbr_agg(const __grid_constant__ GbLayout L, const __grid_constant__ GbBatch Bt, const __grid_constant__ GbRadixDev R, const __grid_constant__ GbDenseDev D, unsigned S) {
-    constexpr int NST = GBR_NST, CR = GBR_NCT, NC = ROWW - 1;      // one record per consumer thread and stage
+    constexpr int NST = gbr_nst<ROWW, PACK>(), CR = GBR_NCT, NC = ROWW - 1, RW = gbr_rw<ROWW, PACK>();      // one record per consumer thread and stage
     extern __shared__ __align__(128) uint64_t gbr_smem2[];
     uint64_t* ring = gbr_smem2;                                       // NST x CR records
-    uint64_t* tkey = ring + (size_t)NST * CR * ROWW;                  // S keys
+    uint64_t* tkey = ring + (size_t)GBR_NST * CR * ROWW;              // S keys
     uint64_t* tacc = tkey + S;                                        // n_words planes of S
     unsigned* tlen = reinterpret_cast<unsigned*>(tacc + (size_t)L.n_words * S);
     __shared__ uint64_t full[NST], empty[NST];
     __shared__ unsigned s_used, s_base;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, B = 1 << R.logB;
-    if (*R.status == 2) return;                 // pass 1 overflowed a stream (every warp, the producer's included): the batch is redone
+    if (*R.status & (GBR_ST_STREAM | GBR_ST_UNFIT)) return;      // pass 1 failed (every warp, the producer's included): the batch is redone
     if (tid == 0) { for (int s = 0; s < NST; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], GBR_NCW); } mbar_fence_init(); }
     __syncthreads();
     if (warp == GBR_NCW) {                      // producer warp: keeps the ring full across bucket boundaries
@@ -398,15 +441,15 @@ __global__ void __launch_bounds__(1024) k_gbr_agg(const __grid_constant__ GbLayo
             unsigned q = 0;
             for (int p = blockIdx.x; p < B; p += gridDim.x) {
                 const int64_t rows = (int64_t)R.cursor[p];
-                const uint64_t* src = R.recs + R.off[p] * ROWW;
+                const uint64_t* src = R.recs + R.off[p] * RW;
                 const int nch = (int)((rows + CR - 1) / CR);
                 for (int c = 0; c < nch; c++, q++) {
                     const int st = q % NST; const unsigned use = q / NST;
                     if (use > 0) while (!mbar_try_wait(&empty[st], (use - 1) & 1u)) {}
                     const int64_t crow = min((int64_t)CR, rows - (int64_t)c * CR);
-                    const unsigned bytes = (unsigned)(((crow + 1) & ~(int64_t)1) * ROWW * 8);      // whole 16-byte units (the buffer is padded)
+                    const unsigned bytes = (unsigned)(((crow + 1) & ~(int64_t)1) * RW * 8);      // whole 16-byte units (the buffer is padded)
                     mbar_expect_tx(&full[st], bytes);
-                    bulk_g2s(ring + (size_t)st * CR * ROWW, src + (size_t)c * CR * ROWW, bytes, &full[st]);
+                    bulk_g2s(ring + (size_t)st * CR * RW, src + (size_t)c * CR * RW, bytes, &full[st]);
                 }
             }
         }
@@ -423,13 +466,13 @@ __global__ void __launch_bounds__(1024) k_gbr_agg(const __grid_constant__ GbLayo
         for (int c = 0; c < nch; c++, q++) {
             const int st = q % NST; const unsigned par = (q / NST) & 1u;
             while (!mbar_try_wait(&full[st], par)) {}
-            const uint64_t* buf = ring + (size_t)st * CR * ROWW;
+            const uint64_t* buf = ring + (size_t)st * CR * RW;
             const int crow = (int)min((int64_t)CR, rows - (int64_t)c * CR);
-            uint64_t rec[ROWW];
-            rec[0] = GB_EMPTY;
+            uint64_t rec[RW];
+            rec[0] = PACK ? GBR_PK_PAD : GB_EMPTY;
             if (tid < crow) {
 #pragma unroll
-                for (int w = 0; w < ROWW; w++) rec[w] = buf[tid * ROWW + w];
+                for (int w = 0; w < RW; w++) rec[w] = buf[tid * RW + w];
             }
             // the release below lets the producer's next TMA write overwrite this stage.  The warp signals before it uses
             // the record, so nothing else waits for these loads: without the proxy fence, a copy issued on lane 0's arrival
@@ -438,8 +481,8 @@ __global__ void __launch_bounds__(1024) k_gbr_agg(const __grid_constant__ GbLayo
             fence_async_smem();
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty[st]);
-            const uint64_t key = rec[0];
-            if (key == GB_EMPTY) continue;              // pad record
+            if (PACK ? (uint32_t)rec[0] == GBR_PK_PAD : rec[0] == GB_EMPTY) continue;      // pad record
+            const uint64_t key = PACK ? R.pk_base + (uint32_t)rec[0] : rec[0];
             unsigned slot = __umulhi((unsigned)((table_hash(key) << R.logB) >> 32), S);
             bool found = false;
             for (unsigned probes = 0; probes < 128u; probes++) {
@@ -453,12 +496,13 @@ __global__ void __launch_bounds__(1024) k_gbr_agg(const __grid_constant__ GbLayo
                 }
                 if (++slot == S) slot = 0;
             }
-            if (!found) { *R.status = 1; continue; }    // more groups in this bucket than its table holds: the caller falls back
+            if (!found) { atomicOr(R.status, GBR_ST_TABLE); continue; }      // more groups in this bucket than its table holds: the caller falls back
             if (L.need_len) atomicAdd(tlen + slot, 1u);
 #pragma unroll
             for (int cix = 0; cix < NC; cix++) {
                 const int dt = Bt.cols[cix].dtype;
-                for (int kk = L.col_kbegin[cix]; kk < L.col_kbegin[cix + 1]; kk++) gb_apply_smem<false>(L.wop[kk], tacc + (size_t)L.wslot[kk] * S + slot, dt, rec[1 + cix], true);
+                const uint64_t raw = PACK && cix == 0 ? gbr_unpack_value(R, rec[0]) : rec[PACK ? cix : 1 + cix];
+                for (int kk = L.col_kbegin[cix]; kk < L.col_kbegin[cix + 1]; kk++) gb_apply_smem<false>(L.wop[kk], tacc + (size_t)L.wslot[kk] * S + slot, dt, raw, true);
             }
         }
         named_bar_sync(1, GBR_NCT);
@@ -473,7 +517,7 @@ __global__ void __launch_bounds__(1024) k_gbr_agg(const __grid_constant__ GbLayo
             if (used) at = atomicSub(&s_used, 1u) - 1u;
             if (used) {
                 const unsigned long long pos = base + at;
-                if ((int64_t)pos >= D.Gb) *R.status = 1;
+                if ((int64_t)pos >= D.Gb) atomicOr(R.status, GBR_ST_TABLE);
                 else {
                     D.keys[pos] = tkey[i]; D.len[pos] = tlen[i]; D.first[pos] = 0xFFFFFFFFu;
                     for (int w = 0; w < L.n_words; w++) D.words[(int64_t)w * D.Gb + pos] = tacc[(size_t)w * S + i];
@@ -503,27 +547,27 @@ static size_t gbr_scatter_smem(int B, int roww, bool bulk) {
     return (tile + (bulk ? B : 0)) * roww * 8 + (size_t)3 * B * 4 + (bulk ? 0 : tile * 2);
 }
 // write-combining scatter: grid = the CTAs that fit at once (persistent; k_gbr_offsets pads for each of them)
-template <int ROWW, int KEY_ELEM, int KEY_CANON>
+template <int ROWW, int KEY_ELEM, int KEY_CANON, bool PACK>
 static int scatter_wc_grid(int B) {
-    auto kfn = k_gbr_scatter_wc<ROWW, KEY_ELEM, KEY_CANON>;
-    const size_t smem = gbr_wc_smem(B, ROWW);
+    auto kfn = k_gbr_scatter_wc<ROWW, KEY_ELEM, KEY_CANON, PACK>;
+    const size_t smem = gbr_wc_smem(B, gbr_rw<ROWW, PACK>());
     PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     PLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kfn, GBR_WC_THREADS, smem));
     return ctx().sm_count * std::max(occ, 1);
 }
-template <int ROWW, int KEY_ELEM, int KEY_CANON>
+template <int ROWW, int KEY_ELEM, int KEY_CANON, bool PACK>
 static void launch_scatter(const GbLayout& L, const GbBatch& Bt, const GbRadixDev& R, bool bulk) {
-    const size_t smem = gbr_scatter_smem(1 << R.logB, ROWW, bulk);
-    auto kfn = bulk ? k_gbr_scatter<ROWW, KEY_ELEM, KEY_CANON, true> : k_gbr_scatter<ROWW, KEY_ELEM, KEY_CANON, false>;
+    const size_t smem = gbr_scatter_smem(1 << R.logB, gbr_rw<ROWW, PACK>(), bulk);
+    auto kfn = bulk ? k_gbr_scatter<ROWW, KEY_ELEM, KEY_CANON, true, PACK> : k_gbr_scatter<ROWW, KEY_ELEM, KEY_CANON, false, PACK>;
     PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     PLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kfn, GBR_THREADS, smem));
     PLB_LAUNCH("k5r_scatter", kfn, ctx().sm_count * std::max(occ, 1), GBR_THREADS, smem, L, Bt, R);
 }
-template <int ROWW>
+template <int ROWW, bool PACK>
 static void launch_agg(const GbLayout& L, const GbBatch& Bt, const GbRadixDev& R, const GbDenseDev& D, unsigned S) {
-    auto kfn = k_gbr_agg<ROWW>;
+    auto kfn = k_gbr_agg<ROWW, PACK>;
     const size_t smem = (size_t)GBR_NST * GBR_NCT * ROWW * 8 + (size_t)S * (8 + 4 + 8 * L.n_words) + 16;      // ring + table
     PLB_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
@@ -542,9 +586,21 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
         if (v == nullptr || v->len != key.len || v->dtype != plans[i].in_dtype || v->validity != nullptr) return false;
         if (dtype_size(v->dtype) != 4 && dtype_size(v->dtype) != 8) return false;
     }
+    // packed records (GbRadixDev): the key in the sampled window (pack_key: integer keys only) and one value column that
+    // fits 32 bits, by dtype (4-byte columns, preferred: no row can miss) or by its sampled range (pack_cols); bound as
+    // column 0.  The plan below (buckets, table, store path, stream sizing) stays the one of the plain width.
+    const void* pk_col = nullptr;
+    if (pack_key && knob_int("BL_K5R_PACK", 1) != 0 && (key.dtype == BL_INT64 || key.dtype == BL_UINT64 || key.dtype == BL_INT32 || key.dtype == BL_UINT32))
+        for (size_t i = 0; i < plans.size(); i++) {
+            if (plans[i].kind == BL_AGG_LEN) continue;
+            const void* v = values[i]->v();
+            if (dtype_size(values[i]->dtype) == 4) { pk_col = v; break; }
+            if (!pk_col && std::find(pack_cols.begin(), pack_cols.end(), v) != pack_cols.end()) pk_col = v;
+        }
     GbBatch Bt; GbLayout Lb;
-    if (!bind_columns(key, values, 0, 0, 4, Bt, Lb)) return false;
+    if (!bind_columns(key, values, 0, 0, 4, Bt, Lb, pk_col)) return false;
     const int roww = 1 + Lb.n_cols;
+    bool pack = pk_col != nullptr;
     const int64_t n = key.len;
     // shared-memory table per bucket: what is left of ~110 KB (2 CTAs / SM) after a
     // 2-stage ring; when even 8192 buckets of that size cannot take the estimated groups, one CTA / SM with a ~200 KB table
@@ -580,10 +636,16 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
     else if (store == 2 && wc_fits) { bulk = false; wc = true; }
     else if (store == 3 && gbr_scatter_smem(B, roww, true) <= (size_t)smem_optin) { bulk = true; wc = false; }
     const int64_t ntiles = (n + GBR_THREADS * GBR_RPT - 1) / (GBR_THREADS * GBR_RPT);
-    // f(KEY_ELEM, KEY_CANON, ROWW) of the scatter kernels for this batch
-    auto with_scatter_form = [&](auto f) { with_key_form(key.dtype, [&](auto e, auto c) { with_at_least<1, 2, 3, 4, 5>(roww, [&](auto w) { f(e, c, w); }); }); };
+    // f(KEY_ELEM, KEY_CANON, ROWW, PACK) of the scatter kernels for this batch (packed forms: integer keys, value columns)
+    auto with_scatter_form = [&](bool pk, auto f) {
+        with_key_form(key.dtype, [&](auto e, auto c) { constexpr bool int_key = decltype(c)::value == 0; with_at_least<1, 2, 3, 4, 5>(roww, [&](auto w) {
+            if constexpr (int_key && decltype(w)::value >= 2) { if (pk) { f(e, c, w, std::true_type{}); return; } }
+            f(e, c, w, std::false_type{});
+        }); });
+    };
+    // the grid (and so the padding) of the plain form, whichever form runs
     int wc_grid = 0;
-    if (wc) with_scatter_form([&](auto e, auto c, auto w) { wc_grid = scatter_wc_grid<decltype(w)::value, decltype(e)::value, decltype(c)::value>(B); });
+    if (wc) with_scatter_form(false, [&](auto e, auto c, auto w, auto) { wc_grid = scatter_wc_grid<decltype(w)::value, decltype(e)::value, decltype(c)::value, false>(B); });
     // worst-case padding of a bucket stream (gbr_stream_records): one record per tile for the runs, F - 1 per CTA for the
     // write-combining buffers, none for the coalesced store
     const unsigned long long pad_units = wc ? (unsigned long long)wc_grid : (unsigned long long)ntiles;
@@ -605,6 +667,7 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
     } catch (const Error&) { cudaGetLastError(); return false; }       // not enough free HBM for the record streams
     GbRadixDev R; memset(&R, 0, sizeof R);
     R.recs = as<uint64_t>(recs); R.logB = logB; R.roww = roww; R.status = as<int>(status);
+    R.pk_base = pack_base; R.pk_sext = Bt.cols[0].dtype == BL_INT64;
     char* cp = reinterpret_cast<char*>(ctl->p);
     R.off = reinterpret_cast<unsigned long long*>(cp); cp += (size_t)(B + 1) * 8;
     R.special = reinterpret_cast<uint64_t*>(cp); cp += (size_t)(1 + GB_MAX_WORDS) * 8;
@@ -626,19 +689,31 @@ bool GroupByState::consume_radix(const DevCol& key, const std::vector<const DevC
         }
         PLB_LAUNCH("k5r_setup", k_gbr_offsets, 1, 1024, 0, L, bucket_rows ? nullptr : R.counts, bucket_rows, B, pad_units, pad_each, align,
                    const_cast<unsigned long long*>(R.off), R.cursor, R.special, R.status);
-        with_scatter_form([&](auto e, auto c, auto w) {
+        with_scatter_form(pack, [&](auto e, auto c, auto w, auto pk) {
             constexpr int E = decltype(e)::value, C = decltype(c)::value, ROWW = decltype(w)::value;
-            if (wc) PLB_LAUNCH("k5r_scatter", (k_gbr_scatter_wc<ROWW, E, C>), wc_grid, GBR_WC_THREADS, gbr_wc_smem(B, ROWW), Lb, Bt, R);
-            else launch_scatter<ROWW, E, C>(Lb, Bt, R, bulk);
+            constexpr bool P = decltype(pk)::value;
+            if (wc) {
+                if (P) (void)scatter_wc_grid<ROWW, E, C, P>(B);      // sets the packed form's shared-memory limit
+                PLB_LAUNCH("k5r_scatter", (k_gbr_scatter_wc<ROWW, E, C, P>), wc_grid, GBR_WC_THREADS, gbr_wc_smem(B, gbr_rw<ROWW, P>()), Lb, Bt, R);
+            }
+            else launch_scatter<ROWW, E, C, P>(Lb, Bt, R, bulk);
         });
         dev_memset(dense.ctl->p, 0, 8); dev_memset(static_cast<char*>(dense.ctl->p) + 8, 0xFF, 8);      // {0, -1}
-        with_at_least<1, 2, 3, 4, 5>(roww, [&](auto w) { launch_agg<decltype(w)::value>(Lb, Bt, R, D, S); });
+        with_at_least<1, 2, 3, 4, 5>(roww, [&](auto w) { with_bool(pack, [&](auto pk) {
+            constexpr int ROWW = decltype(w)::value;
+            if constexpr (ROWW >= 2 || !decltype(pk)::value) launch_agg<ROWW, decltype(pk)::value>(Lb, Bt, R, D, S);
+        }); });
         PLB_LAUNCH("k5r_special", k_gbr_append_special, 1, 32, 0, R.special, L.n_words, D, as<int>(status));
         const int st = read_scalar(as<int>(status));      // also orders the recs lifetime
         if (getenv("BL_K5_DEBUG"))
-            fprintf(stderr, "[k5r] rows=%lld est_groups=%lld buckets=%d slots=%u bulk=%d store=%s sizing=%s cap=%llu status=%d\n", (long long)n, (long long)est_groups, B, S, (int)bulk,
-                    bulk ? "runs" : wc ? "wc" : "coalesced", bucket_rows ? "sample" : "exact", cap, st);
-        if (st == 2 && bucket_rows) {       // a bucket outgrew its sampled stream: once more with exact sizing
+            fprintf(stderr, "[k5r] rows=%lld est_groups=%lld buckets=%d slots=%u bulk=%d store=%s sizing=%s cap=%llu packed=%d status=%d\n", (long long)n, (long long)est_groups, B, S,
+                    (int)bulk, bulk ? "runs" : wc ? "wc" : "coalesced", bucket_rows ? "sample" : "exact", cap, (int)pack, st);
+        // pass 1 failed: once more with plain records (a row outside the packed form) and / or exact sizing (a bucket
+        // outgrew its sampled stream), both in the same redo
+        const bool unfit = st & GBR_ST_UNFIT, overflow = st & GBR_ST_STREAM;
+        if ((unfit || overflow) && (!unfit || pack) && (!overflow || bucket_rows)) {
+            if (unfit) pack = false;
+            if (!overflow) continue;
             bucket_rows = 0;
             if (exact_rows > rec_rows) {
                 recs.reset();
