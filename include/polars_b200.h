@@ -324,6 +324,31 @@ bl_status bl_arg_sort_keys(const bl_sort_key* by, int32_t n_by, int64_t limit, i
  * key dtype bl_arg_sort does not take: BL_ERR_UNSUPPORTED; more than 2^32 - 1 rows: BL_ERR_UNSUPPORTED. */
 bl_status bl_top_k(const bl_sort_key* by, int32_t n_by, int64_t k, int32_t out_location, bl_column* out_idx);
 
+/* ---- unique  (DataFrame::unique_impl polars-core/src/frame/mod.rs:2317-2392; is_unique / is_duplicated frame/mod.rs:2408-2442,
+ * polars-ops/src/series/ops/is_unique.rs:11-41,113-119; is_first_distinct.rs:107-161; is_last_distinct.rs:12-…) -------- */
+enum { BL_UNIQUE_FIRST = 0, BL_UNIQUE_LAST = 1, BL_UNIQUE_ANY = 2, BL_UNIQUE_NONE = 3 };
+enum { BL_DISTINCT_FIRST = 0, BL_DISTINCT_LAST = 1, BL_DISTINCT_UNIQUE = 2, BL_DISTINCT_DUPLICATED = 3 };
+/* The rows DataFrame.unique(subset, keep, maintain_order, slice) keeps, as UInt32 row ids in ASCENDING ROW ORDER.  The
+ * reference: First / Any with maintain_order take each key's first row in first-occurrence order; Last with maintain_order
+ * takes the keys' last rows sorted ascending; None is filter(is_unique); without maintain_order the same rows come in an
+ * open order.  Row order is therefore exact for maintain_order and a valid order otherwise; a `slice` (offset, len) is that
+ * sub-range of the ids.  BL_UNIQUE_ANY is BL_UNIQUE_FIRST.  Key equality as group_by: null is a value of its own, floats
+ * compare by total equality (-0.0 == +0.0, every NaN equal), strings by bytes, several columns form one row key; a kept row
+ * keeps its own bytes (on [+0.0, -0.0] FIRST keeps +0.0 and LAST -0.0).  Empty input: no rows.
+ * subset: one bl_sort_key per key column with flags 0: numeric / Boolean (one chunk) or LargeUtf8 / LargeBinary.
+ * Plan (DESIGN.md §18): the K5 table with each key's first row and row count, one more pass for the last rows (LAST only),
+ * one pass that marks the kept rows in a bitmap, its compaction.  Device memory: the K5 table, 4 B per table slot for the
+ * last rows (LAST only), n / 8 B of mask, the ids; string keys add their codes (4 B per row).
+ * Errors: an unknown keep, flags != 0, a descriptor with both or neither pointer set, n_subset < 1, null pointers, key
+ * columns of different lengths: BL_ERR_INVALID; another key dtype: BL_ERR_UNSUPPORTED; more than 2^32 - 2 rows:
+ * BL_ERR_UNSUPPORTED (checked before any upload). */
+bl_status bl_unique(const bl_sort_key* subset, int32_t n_subset, int32_t keep, int32_t out_location, bl_column* out_idx);
+/* One Boolean per row (BL_BOOL, n rows, no nulls) over the same keys: BL_DISTINCT_FIRST = is_first_distinct (the row is its
+ * key's first), BL_DISTINCT_LAST = is_last_distinct (its key's last), BL_DISTINCT_UNIQUE = is_unique (the key occurs once),
+ * BL_DISTINCT_DUPLICATED = is_duplicated (more than once).  Arguments, errors and memory as bl_unique; an unknown kind:
+ * BL_ERR_INVALID. */
+bl_status bl_unique_mask(const bl_sort_key* keys, int32_t n_keys, int32_t kind, int32_t out_location, bl_column* out_mask);
+
 /* ---- asof join  (_join_asof_dispatch polars-ops/src/frame/join/asof/mod.rs:325-394; by keys groups.rs:39-345) ------- */
 enum { BL_ASOF_BACKWARD = 0, BL_ASOF_FORWARD = 1, BL_ASOF_NEAREST = 2 };
 /* The reference's take_idx: out_right_idx (BL_UINT32, left_on->length rows, nullable; a null slot holds BL_IDX_NULL) names,

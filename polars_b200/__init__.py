@@ -818,6 +818,73 @@ def bottom_k_by(cols: Sequence, by, k: int, reverse=False, location: int = HOST)
     return _select_sorted(cols, by, k, _reverse_flags(by, reverse), location)
 
 
+UNIQUE_KEEP = {"first": 0, "last": 1, "any": 2, "none": 3}
+DISTINCT_KINDS = {"first": 0, "last": 1, "unique": 2, "duplicated": 3}
+
+
+def _unique_key_descs(keys):
+    """one key column or a list of them (numeric / Boolean, or string columns as _by_key takes them) -> (bl_sort_key
+    array, the objects it points into)"""
+    ks = keys if isinstance(keys, list) else [keys]
+    keep = []
+    return (BlSortKey * len(ks))(*[_by_key(k, keep) for k in ks]), keep
+
+
+def arg_unique(keys, keep: str = "first", location: int = HOST):
+    """bl_unique: the rows DataFrame.unique(subset=keys, keep=keep) keeps, as UInt32 row ids in ascending ROW order.
+    keep: "first" / "any" (each key's first row; "any" is "first"), "last" (each key's last row) or "none" (only the rows
+    whose key occurs once).  There is no `maintain_order`: row order is what maintain_order=True gives and a valid order
+    when it is False.  Host output: a numpy uint32 array; device output: an OutColumn."""
+    if keep not in UNIQUE_KEEP:
+        raise ValueError(f"`keep` must be one of {{'first', 'last', 'any', 'none'}}, got {keep}")
+    descs, hold = _unique_key_descs(keys)
+    out = BlColumn()
+    _check(lib().bl_unique(descs, C.c_int32(len(descs)), C.c_int32(UNIQUE_KEEP[keep]), C.c_int32(location), C.byref(out)))
+    res = _finish([out], location)[0]
+    return res[0] if location == HOST else res
+
+
+def unique(cols: Sequence, subset=None, keep: str = "any", location: int = HOST):
+    """DataFrame.unique(subset, keep): the columns `cols` at arg_unique(cols[subset], keep), in row order (what
+    maintain_order=True gives; there is no `maintain_order` parameter).  subset: indices into `cols`, None = every column.
+    Numeric columns go through gather, string columns through string_gather.  Returns a list like `gather` returns."""
+    if keep not in UNIQUE_KEEP:
+        raise ValueError(f"`keep` must be one of {{'first', 'last', 'any', 'none'}}, got {keep}")
+    idx = range(len(cols)) if subset is None else subset
+    ids = arg_unique([cols[i] for i in idx], keep, location=DEVICE)
+    nums = [c for c in cols if not _is_string_key(c)]
+    got = iter(gather(nums, ids, check_bounds=False, location=location) if nums else [])
+    return [string_gather(c, ids, location=location) if _is_string_key(c) else next(got) for c in cols]
+
+
+def _unique_mask(keys, kind: str, location: int):
+    descs, hold = _unique_key_descs(keys)
+    out = BlColumn()
+    _check(lib().bl_unique_mask(descs, C.c_int32(len(descs)), C.c_int32(DISTINCT_KINDS[kind]), C.c_int32(location), C.byref(out)))
+    res = _finish([out], location)[0]
+    return res[0] if location == HOST else res
+
+
+def is_unique(keys, location: int = HOST):
+    """is_unique: True where the row's key (one column or a list of them) occurs once.  Host output: a numpy bool array."""
+    return _unique_mask(keys, "unique", location)
+
+
+def is_duplicated(keys, location: int = HOST):
+    """is_duplicated: True where the row's key occurs more than once."""
+    return _unique_mask(keys, "duplicated", location)
+
+
+def is_first_distinct(keys, location: int = HOST):
+    """is_first_distinct: True where the row is the first with its key."""
+    return _unique_mask(keys, "first", location)
+
+
+def is_last_distinct(keys, location: int = HOST):
+    """is_last_distinct: True where the row is the last with its key."""
+    return _unique_mask(keys, "last", location)
+
+
 ASOF_STRATEGIES = {"backward": 0, "forward": 1, "nearest": 2}
 
 

@@ -185,6 +185,8 @@ bool sortable_dtype(int dt);      // the key dtypes op_arg_sort and op_top_k tak
 // the first k rows of op_arg_sort's stable order, as ascending UInt32 row ids (top_k.cu)
 DevCol op_top_k(const std::vector<DevCol>& by, const std::vector<int>& flags, int64_t k);
 DevCol op_mask_rows(const uint32_t* mask, int64_t n);      // the ascending row ids of the set bits (filter.cu)
+// the BL_DISTINCT_* mask of the rows keyed by cols (numeric / Boolean columns or string codes; unique.cu): BL_BOOL, no nulls
+DevCol op_unique_mask(const std::vector<DevCol>& cols, int kind);
 void mask_first_into(const uint32_t* mask, int64_t n, int64_t count, uint32_t* out);      // out |= the first `count` set bits of mask (filter.cu)
 // bl_sort_key descriptors -> key columns (string keys as their ascending dense rank) and flags; who: the message prefix
 void import_sort_key_list(const bl_sort_key* by, int32_t n_by, const char* who, std::vector<DevCol>& keys, std::vector<int>& flags);

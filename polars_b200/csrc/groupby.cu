@@ -1639,23 +1639,8 @@ void GroupByState::finish(bool maintain_order, const DevCol* key_col_for_gather,
 //   3. stable radix sort of (first-of-group, row): groups in first-occurrence order, rows ascending
 //   4. run starts of the sorted keys -> offsets, first = all[offsets]
 __global__ void __launch_bounds__(256) k_gb_lookup_first(const __grid_constant__ GbTableDev T, const void* keys, const uint32_t* key_validity, int key_dtype, int64_t n, uint32_t* __restrict__ out) {
-    const uint64_t mask = T.cap - 1;
-    for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < n; row += (int64_t)gridDim.x * blockDim.x) {
-        const bool kvalid = key_validity == nullptr || bit_get(key_validity, row);
-        const uint64_t key = load_key_rt(keys, key_dtype, row);
-        uint64_t slot;
-        if (!kvalid) slot = T.cap;
-        else if (key == GB_EMPTY) slot = T.cap + 1;
-        else {
-            slot = table_hash(key) >> T.shift;
-            for (int probes = 0; probes < GB_MAX_PROBE; ++probes) {
-                if (__ldcg(reinterpret_cast<const unsigned long long*>(T.entries + slot * T.es)) == key) break;
-                slot = (slot + 1) & mask;
-            }
-        }
-        const uint64_t w1 = __ldcg(reinterpret_cast<const unsigned long long*>(T.entries + slot * T.es + gb_woff((int64_t)slot, 1, T.ws, T.pw)));
-        out[row] = (uint32_t)(w1 >> 32);
-    }
+    for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < n; row += (int64_t)gridDim.x * blockDim.x)
+        out[row] = (uint32_t)(gb_slot_word1(T, gb_lookup_slot(T, keys, key_validity, key_dtype, row)) >> 32);
 }
 // bit i of the mask = sorted[i] starts a run (i == 0 or sorted[i] != sorted[i-1]); n_round = n rounded up to 32
 __global__ void __launch_bounds__(256) k_run_starts(const uint32_t* __restrict__ sorted, int64_t n, int64_t n_round, uint32_t* __restrict__ mask_words) {

@@ -31,6 +31,25 @@ __device__ __forceinline__ uint64_t load_key_rt(const void* keys, int dtype, int
     }
 }
 
+// the slot of a row's key in a built table, by the build's rules: a null key -> cap, the GB_EMPTY key -> cap + 1, any other
+// key -> linear probing from its hash (k_gb_lookup_first, unique.cu)
+__device__ __forceinline__ uint64_t gb_lookup_slot(const GbTableDev& T, const void* keys, const uint32_t* key_validity, int key_dtype, int64_t row) {
+    if (key_validity != nullptr && !bit_get(key_validity, row)) return T.cap;
+    const uint64_t key = load_key_rt(keys, key_dtype, row);
+    if (key == GB_EMPTY) return T.cap + 1;
+    const uint64_t mask = T.cap - 1;
+    uint64_t slot = table_hash(key) >> T.shift;
+    for (int probes = 0; probes < GB_MAX_PROBE; ++probes) {
+        if (__ldcg(reinterpret_cast<const unsigned long long*>(T.entries + slot * T.es)) == key) break;
+        slot = (slot + 1) & mask;
+    }
+    return slot;
+}
+// word 1 of a slot: lo32 = len, hi32 = first row
+__device__ __forceinline__ uint64_t gb_slot_word1(const GbTableDev& T, uint64_t slot) {
+    return __ldcg(reinterpret_cast<const unsigned long long*>(T.entries + slot * T.es + gb_woff((int64_t)slot, 1, T.ws, T.pw)));
+}
+
 
 __device__ __forceinline__ double raw_to_f64(int dtype, uint64_t raw) {
     switch (dtype) {

@@ -141,7 +141,7 @@ static void release_inputs(SeriesExport* inputs, size_t n) {
     }
 }
 
-enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER, P_ROLL, P_ROLL_BY, P_RANK, P_ROLL_Q, P_ROLL_Q_BY, P_TOP_K };
+enum PluginOp { P_ARITH, P_CMP, P_FILTER, P_GATHER, P_GROUP, P_JOIN, P_SORT, P_OVER, P_ROLL, P_ROLL_BY, P_RANK, P_ROLL_Q, P_ROLL_Q_BY, P_TOP_K, P_UNIQUE, P_DISTINCT };
 
 // ---- kwargs ----------------------------------------------------------------------------------------
 // register_plugin_function(kwargs={...}) pickles the dict (py-polars/src/polars/plugins.py:100-115) and the caller hands
@@ -239,7 +239,7 @@ static void require_int_kwargs(std::initializer_list<double> vs, const char* who
 static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, const Kwargs& kw, SeriesExport* ret) {
     std::lock_guard<std::recursive_mutex> lk(ctx().mu);
     PLB_REQUIRE(n >= 1, BL_ERR_INVALID, "plugin: no input series");
-    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER && kind != P_ROLL && kind != P_ROLL_BY && kind != P_RANK && kind != P_ROLL_Q && kind != P_ROLL_Q_BY && kind != P_TOP_K) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
+    if (kind != P_GROUP && kind != P_JOIN && kind != P_SORT && kind != P_OVER && kind != P_ROLL && kind != P_ROLL_BY && kind != P_RANK && kind != P_ROLL_Q && kind != P_ROLL_Q_BY && kind != P_TOP_K && kind != P_UNIQUE && kind != P_DISTINCT) PLB_REQUIRE(n == 2, BL_ERR_INVALID, "plugin: expected exactly 2 input series");
     std::vector<std::vector<bl_column>> chunks(n);
     std::vector<DevCol> in;
     for (size_t i = 0; i < n; i++) { int dt; chunks[i] = input_chunks(inputs[i], &dt); in.push_back(import_column(chunks[i].data(), (int)chunks[i].size())); }
@@ -281,6 +281,24 @@ static void run_plugin(PluginOp kind, int op, SeriesExport* inputs, size_t n, co
             bl_column h; export_column(perm, BL_HOST, &h);
             fill_array(array, h);
             fill_schema(schema, name, format_of(BL_UINT32));
+        } else if (kind == P_UNIQUE || kind == P_DISTINCT) {
+            // inputs: the key columns (numeric or Boolean).  bl_arg_unique -> the kept rows as ascending UInt32 row ids, kwarg
+            // keep ("first" (default), "last", "any", "none"); bl_is_* -> one Boolean per row
+            int mk = op;
+            if (kind == P_UNIQUE) {
+                const std::string keep = kw.gets("keep", "first");
+                static const char* names[] = {"first", "last", "any", "none"};      // BL_UNIQUE_FIRST .. BL_UNIQUE_NONE
+                int k = -1;
+                for (int j = 0; j < 4; j++) if (keep == names[j]) k = j;
+                PLB_REQUIRE(k >= 0, BL_ERR_INVALID, "`keep` must be one of {'first', 'last', 'any', 'none'}, got " + keep);
+                mk = k == BL_UNIQUE_LAST ? BL_DISTINCT_LAST : k == BL_UNIQUE_NONE ? BL_DISTINCT_UNIQUE : BL_DISTINCT_FIRST;
+            }
+            for (auto& c : in) PLB_REQUIRE(sortable_dtype(c.dtype), BL_ERR_UNSUPPORTED, std::string("plugin unique: key dtype ") + dtype_name(c.dtype) + " is not supported");
+            DevCol o = op_unique_mask(in, mk);
+            if (kind == P_UNIQUE) o = op_mask_rows(as<uint32_t>(o.values), o.len);
+            bl_column h; export_column(o, BL_HOST, &h);
+            fill_array(array, h);
+            fill_schema(schema, name, format_of(o.dtype));
         } else if (kind == P_TOP_K) {
             // inputs: the `by` columns -> the UInt32 ids of the first k rows, best first (DataFrame.top_k / bottom_k:
             // descending = !reverse for top (op 0), reverse for bottom (op 1), nulls last).  kwargs: k (int, required),
@@ -478,7 +496,8 @@ static void field_entry(PluginOp kind, int op, const ArrowSchema* fields, size_t
     switch (kind) {
         case P_ARITH: fill_schema(out, name, format_of((op == BL_OP_TRUE_DIV && dt >= 0 && dt <= BL_UINT64) ? BL_FLOAT64 : (dt < 0 ? BL_INT64 : dt))); break;
         case P_CMP: fill_schema(out, name, "b"); break;
-        case P_SORT: case P_TOP_K: fill_schema(out, name, format_of(BL_UINT32)); break;
+        case P_SORT: case P_TOP_K: case P_UNIQUE: fill_schema(out, name, format_of(BL_UINT32)); break;
+        case P_DISTINCT: fill_schema(out, name, "b"); break;
         case P_OVER: fill_schema(out, name, format_of(over_scan_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_ROLL: fill_schema(out, name, format_of(rolling_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
         case P_ROLL_BY: fill_schema(out, name, format_of(rolling_dtype(op, dt < 0 ? BL_INT64 : dt))); break;
@@ -552,6 +571,11 @@ PLUGIN(join_anti_idx, P_JOIN, BL_JOIN_ANTI)
 PLUGIN(arg_sort, P_SORT, 0)                     /* kwargs: descending, nulls_last (bool or bitmask); inputs = by columns */
 PLUGIN(top_k_idx, P_TOP_K, 0)                   /* kwargs: k, reverse (bool or bitmask); inputs = by columns */
 PLUGIN(bottom_k_idx, P_TOP_K, 1)
+PLUGIN(arg_unique, P_UNIQUE, 0)                 /* kwargs: keep (default "first"); inputs = key columns */
+PLUGIN(is_unique, P_DISTINCT, BL_DISTINCT_UNIQUE)
+PLUGIN(is_duplicated, P_DISTINCT, BL_DISTINCT_DUPLICATED)
+PLUGIN(is_first_distinct, P_DISTINCT, BL_DISTINCT_FIRST)
+PLUGIN(is_last_distinct, P_DISTINCT, BL_DISTINCT_LAST)
 PLUGIN(cum_sum, P_OVER, BL_CUM_SUM)             /* kwargs: reverse; inputs = values, then partition keys */
 PLUGIN(cum_prod, P_OVER, BL_CUM_PROD)
 PLUGIN(cum_min, P_OVER, BL_CUM_MIN)

@@ -22,6 +22,8 @@ Recognised:
   * Join(inner|left|semi|anti, one key column per side) of two DataFrameScans -> bl_hash_join + bl_gather
   * Sort(by=[col, ...] of numeric / Boolean columns, slice None or (0, k)) of a DataFrameScan -> bl_arg_sort (limit = k)
     + bl_gather of the numeric columns (other columns: Polars' take of the same permutation)
+  * Distinct(keep, subset of numeric / Boolean columns or None, maintain_order, slice) of a DataFrameScan -> bl_unique
+    + bl_gather of the numeric columns (other columns: Polars' take of the same row ids)
 """
 from __future__ import annotations
 
@@ -309,6 +311,78 @@ def _plan_sort(plb, nt, root_id, node):
     return run
 
 
+_KEEP = {"first", "last", "any", "none"}
+
+
+def _distinct_options(options):
+    """Distinct.options = (keep, subset | None, maintain_order, slice | None) (visitor/nodes.rs:678-695); keep is the
+    strategy's snake_case name.  Returns (keep, subset, slice) or raises for a shape the UDF does not take."""
+    if not isinstance(options, (tuple, list)) or len(options) != 4:
+        raise _Unsupported("distinct options")
+    keep, subset, maintain_order, slc = options
+    if not isinstance(keep, str) or keep not in _KEEP or not isinstance(maintain_order, bool):
+        raise _Unsupported(f"distinct keep {keep!r}")
+    if subset is not None and (not isinstance(subset, (tuple, list)) or not subset or not all(isinstance(c, str) for c in subset)):
+        raise _Unsupported("distinct subset")
+    if slc is not None and (not isinstance(slc, (tuple, list)) or len(slc) != 2 or not all(isinstance(v, int) and not isinstance(v, bool) for v in slc)
+                            or slc[1] < 0):
+        raise _Unsupported("distinct slice")
+    return keep, None if subset is None else list(subset), None if slc is None else tuple(slc)
+
+
+def _slice_ids(ids, slc):
+    """the (offset, len) slice of the kept row ids, as the reference's slice_offsets clamps it (a negative offset counts
+    from the end)"""
+    if slc is None:
+        return ids
+    offset, length = slc
+    n = len(ids)
+    start = offset + n if offset < 0 else offset
+    stop = min(max(start + length, 0), n)
+    start = min(max(start, 0), n)
+    return ids[start:stop]
+
+
+def _plan_distinct(plb, nt, root_id, node):
+    """Distinct(input=DataFrameScan, options=(keep, subset, maintain_order, slice)): DataFrame.unique, SELECT DISTINCT,
+    UNION.  The kept rows come from bl_unique in ascending row order, which is what maintain_order asks for and a valid
+    order when it is not set; the slice applies to them.  The subset (every column when None) must be numeric or Boolean,
+    checked on the node's schema: anything else (String, temporal, nested ...) leaves the node to Polars.  The 4- and 8-byte
+    numeric columns are gathered with K4, the others with Polars' own take of the same ids."""
+    keep, subset, slc = _distinct_options(getattr(node, "options", None))
+    if not hasattr(nt, "get_schema"):
+        raise _Unsupported("no schema to check the subset against")
+    schema = {str(k): str(v) for k, v in dict(nt.get_schema()).items()}
+    names = list(schema) if subset is None else subset
+    if not names:
+        raise _Unsupported("distinct over no columns")
+    for c in names:
+        if schema.get(c) not in _SORTABLE:
+            raise _Unsupported(f"distinct key {c}: dtype {schema.get(c)}")
+    frame = _scan_frame(nt, node.input)
+    nt.set_node(root_id)
+
+    def run(*_args: Any, **_kwargs: Any):
+        import polars as pl
+        df = frame().rechunk()
+        ids = _slice_ids(plb.arg_unique([_host_column(df.get_column(c)) for c in (df.columns if subset is None else subset)], keep), slc)
+        dev_cols = [c for c in df.columns if str(df.schema[c]) in _NUMERIC]          # K4 takes 4- and 8-byte elements
+        res = {}
+        if dev_cols:
+            outs = plb.gather([_host_column(df.get_column(c)) for c in dev_cols], np.ascontiguousarray(ids, dtype=np.uint32), check_bounds=False)
+            for c, (v, m) in zip(dev_cols, outs):
+                s = pl.Series(c, v)
+                res[c] = s.set(pl.Series(~m), None) if m is not None else s
+        rest = [c for c in df.columns if c not in res]
+        if rest:
+            taken = df.select(rest)[pl.Series(ids)]
+            for c in rest:
+                res[c] = taken.get_column(c)
+        return pl.DataFrame([res[c] for c in df.columns])
+
+    return run
+
+
 def execute_with_b200(nt: Any, duration_since_start: int | None = None, *, raise_on_fail: bool = False) -> None:
     """The post-optimisation callback.  Leaves the plan untouched when the root is not a supported shape."""
     import polars_b200 as plb
@@ -322,6 +396,8 @@ def execute_with_b200(nt: Any, duration_since_start: int | None = None, *, raise
             fn = _plan_join(plb, nt, root_id, root)
         elif kind == "Sort":
             fn = _plan_sort(plb, nt, root_id, root)
+        elif kind == "Distinct":
+            fn = _plan_distinct(plb, nt, root_id, root)
         else:
             raise _Unsupported(kind)
         nt.set_udf(fn)
