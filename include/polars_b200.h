@@ -240,6 +240,42 @@ bl_status bl_hash_join_strings(const bl_string_column* left_chunks, int32_t n_le
 bl_status bl_string_column_to(const bl_string_column* chunks, int32_t n_chunks, int32_t location, bl_string_column* out);
 void bl_string_column_free(bl_string_column* col);
 
+/* ---- string predicates and filter (DESIGN.md §19) ------------------------------------------------------------------ */
+/* Every result is a BL_BOOL column of the column's length whose validity is the AND of the input validities.  A single
+ * device chunk is read in place (its Arrow offset and a first offset other than 0 included; no byte past offsets[n] is
+ * read); host and multi-chunk inputs are copied to the device first.  A column of length 1 is a scalar.
+ * lhs (op) rhs; rhs has lhs's length or length 1.  Lexicographic unsigned-byte order, a proper prefix first, so
+ * "a" < "a\0" < "b" (polars-compute/src/comparisons/binary.rs:8-70).  A null on either side gives null; a null scalar gives
+ * an all-null column.  missing != 0 (EQ / NE only): eq_missing / ne_missing, null == null is true and the result has no
+ * nulls; against a null scalar that is is_null (EQ) / is_not_null (NE).
+ * Errors: an unknown op, missing with another op, rhs of another length: BL_ERR_INVALID; more than 2^32 - 2 rows:
+ * BL_ERR_UNSUPPORTED (as bl_string_encode). */
+bl_status bl_string_compare(int32_t op, const bl_string_column* lhs, int32_t n_lhs_chunks, const bl_string_column* rhs, int32_t n_rhs_chunks,
+                            int32_t missing, int32_t out_location, bl_column* out);
+enum { BL_STR_STARTS_WITH = 0, BL_STR_ENDS_WITH = 1, BL_STR_CONTAINS = 2, BL_STR_LIKE = 3 };
+/* flags: BL_STR_NEGATE (NOT) flips each valid result, nulls stay null.  LIKE only: BL_LIKE_NO_NEWLINE: '%' and '_' do not
+ * match '\n' (the regex '.' without (?s)); BL_LIKE_OPEN_START / BL_LIKE_OPEN_END: the match may begin / end anywhere, as if
+ * the pattern had a leading / trailing run of any bytes that newlines do not stop (a regex search without '^' / '$'). */
+enum { BL_STR_NEGATE = 1, BL_LIKE_NO_NEWLINE = 2, BL_LIKE_OPEN_START = 4, BL_LIKE_OPEN_END = 8 };
+/* STARTS_WITH / ENDS_WITH / CONTAINS are byte predicates (polars-ops/src/chunked_array/binary/namespace.rs:58-125); on Utf8
+ * columns CONTAINS is str.contains(literal=True) (strings/namespace.rs:174-200, 348-353).  The empty pattern matches every
+ * non-null row; a null scalar pattern gives an all-null column; with a per-row pattern column a null pattern gives a null
+ * row.  Needles of any length.
+ * LIKE is what polars-sql builds for `col LIKE 'pattern'` (sql_expr.rs:435-479, visit_like): ^(?s)<pattern>$ where '%'
+ * matches any run of characters, '_' exactly one character (one UTF-8 sequence, not one byte) and every other byte itself.
+ * LIKE reads the bytes as UTF-8: the ABI cannot tell Utf8 from Binary, and '_' over bytes that are not UTF-8 is undefined.
+ * escape (LIKE only; 0 = none) is an extension the reference rejects: that byte followed by '%', '_' or itself is that
+ * literal byte; followed by anything else, or at the end, it is BL_ERR_INVALID.  The pattern must be a scalar.
+ * Errors: an unknown kind or flag, a BL_LIKE_* flag or escape with another kind, a per-row LIKE pattern, a pattern whose
+ * length is neither 1 nor the column's: BL_ERR_INVALID; a LIKE pattern with more than 63 literal bytes and '_' ('%' is
+ * free): BL_ERR_UNSUPPORTED; more than 2^32 - 2 rows: BL_ERR_UNSUPPORTED. */
+bl_status bl_string_match(int32_t kind, int32_t flags, int32_t escape, const bl_string_column* col, int32_t n_chunks,
+                          const bl_string_column* pattern, int32_t n_pattern_chunks, int32_t out_location, bl_column* out);
+/* The rows whose mask bit is set, in row order (polars-compute/src/filter/mod.rs:18-110); a null mask slot counts as false,
+ * as bl_filter.  mask: BL_BOOL (BL_ERR_DTYPE otherwise) of the column's length (BL_ERR_INVALID otherwise).  More than
+ * 2^32 - 2 rows: BL_ERR_UNSUPPORTED. */
+bl_status bl_string_filter(const bl_string_column* chunks, int32_t n_chunks, const bl_column* mask, int32_t out_location, bl_string_column* out);
+
 /* ---- K7/K8: hash join on one numeric key ----------------------------------------------- */
 /* (build_tables single_keys.rs:16-167, probe_inner single_keys_inner.rs:11-149,
  *  hash_join_tuples_left single_keys_left.rs:106-195) */

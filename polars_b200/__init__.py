@@ -491,6 +491,130 @@ def hash_join_strings(left, right, how: str = "inner", nulls_equal: bool = False
     return tuple(_finish([ol, orr], location))
 
 
+# ---------------------------------------------------------------------------------- string predicates
+STR_KINDS = {"starts_with": 0, "ends_with": 1, "contains": 2, "like": 3}
+STR_NEGATE, LIKE_NO_NEWLINE, LIKE_OPEN_START, LIKE_OPEN_END = 1, 2, 4, 8
+# the characters regex::escape escapes (regex-syntax/src/lib.rs is_meta_character): `\` + one of them is that character
+_RX_META = set("\\.+*?()|[]{}^$#&-~")
+
+
+def _str_chunks(col) -> list:
+    return col if isinstance(col, list) else [col]
+
+
+def _str_operand(x) -> list:
+    """a string column (or list of chunks), or a str / bytes / None scalar as a one-row column"""
+    if x is None or isinstance(x, (str, bytes, bytearray)):
+        return [StringColumn([x])]
+    return _str_chunks(x)
+
+
+def str_compare(op: str, col, other, missing: bool = False, location: int = HOST):
+    """bl_string_compare: col (op) other in unsigned byte order, a proper prefix first.  other: a string column of col's
+    length or a str / bytes / None scalar.  missing: eq_missing / ne_missing.  -> (values, valid) | OutColumn"""
+    lc, rc = _str_chunks(col), _str_operand(other)
+    out = BlColumn()
+    _check(lib().bl_string_compare(C.c_int32(CMPS[op]), _str_array(lc), C.c_int32(len(lc)), _str_array(rc), C.c_int32(len(rc)), C.c_int32(int(missing)),
+                                   C.c_int32(location), C.byref(out)))
+    return _finish([out], location)[0]
+
+
+def _str_match(kind: str, col, pattern, flags: int = 0, escape=None, location: int = HOST):
+    cc, pc = _str_chunks(col), _str_operand(pattern)
+    esc = 0 if escape is None else (ord(escape) if isinstance(escape, str) else int(escape))
+    out = BlColumn()
+    _check(lib().bl_string_match(C.c_int32(STR_KINDS[kind]), C.c_int32(flags), C.c_int32(esc), _str_array(cc), C.c_int32(len(cc)), _str_array(pc), C.c_int32(len(pc)),
+                                 C.c_int32(location), C.byref(out)))
+    return _finish([out], location)[0]
+
+
+def str_starts_with(col, prefix, location: int = HOST):
+    """bl_string_match(STARTS_WITH): prefix is a str / bytes / None scalar or a string column of col's length"""
+    return _str_match("starts_with", col, prefix, location=location)
+
+
+def str_ends_with(col, suffix, location: int = HOST):
+    """bl_string_match(ENDS_WITH): suffix is a str / bytes / None scalar or a string column of col's length"""
+    return _str_match("ends_with", col, suffix, location=location)
+
+
+def str_like(col, pattern, negate: bool = False, no_newline: bool = False, escape=None, location: int = HOST):
+    """bl_string_match(LIKE): SQL `col [NOT] LIKE pattern` as polars-sql evaluates it ('%' any run of characters, '_' one
+    character, newlines included unless no_newline).  escape: an optional escape character for literal '%' / '_'."""
+    flags = (STR_NEGATE if negate else 0) | (LIKE_NO_NEWLINE if no_newline else 0)
+    return _str_match("like", col, pattern, flags, escape, location)
+
+
+def regex_to_device(pattern: str):
+    """Maps a regex of the subset the device takes to (kind, pattern bytes, flags, escape); anything else raises
+    B200Error with status 4 (UNSUPPORTED).  The subset: an optional leading `(?s)`, an optional `^`, then escaped
+    metacharacters, other characters, `.` and `.*`, and an optional `$` — with the regex crate's meaning: `$` matches at
+    the end of the text only, `.` is one character and matches `\\n` only under `(?s)`."""
+    def refuse(why):
+        raise B200Error(4, f"str_contains: the regex {pattern!r} is outside the device subset ({why})")
+    s = pattern
+    dotall = s.startswith("(?s)")
+    if dotall:
+        s = s[4:]
+    anchored_start = s.startswith("^")
+    if anchored_start:
+        s = s[1:]
+    toks, i = [], 0          # ("lit", char) | ("any",) | ("star",)
+    anchored_end = False
+    while i < len(s):
+        ch = s[i]
+        if ch == "\\":
+            if i + 1 >= len(s) or s[i + 1] not in _RX_META:
+                refuse("escape " + s[i:i + 2])
+            toks.append(("lit", s[i + 1]))
+            i += 2
+        elif ch == ".":
+            if i + 1 < len(s) and s[i + 1] == "*":
+                toks.append(("star",))
+                i += 2
+            else:
+                toks.append(("any",))
+                i += 1
+        elif ch == "$" and i == len(s) - 1:
+            anchored_end = True
+            i += 1
+        elif ch in _RX_META:
+            refuse("metacharacter " + ch)
+        else:
+            toks.append(("lit", ch))
+            i += 1
+    if all(t[0] == "lit" for t in toks) and not (anchored_start and anchored_end):
+        lit = "".join(t[1] for t in toks).encode()
+        kind = "starts_with" if anchored_start else "ends_with" if anchored_end else "contains"
+        return kind, lit, 0, None
+    like = "".join(("\\" + t[1] if t[1] in "%_\\" else t[1]) if t[0] == "lit" else "_" if t[0] == "any" else "%" for t in toks)
+    flags = (0 if dotall else LIKE_NO_NEWLINE) | (0 if anchored_start else LIKE_OPEN_START) | (0 if anchored_end else LIKE_OPEN_END)
+    return "like", like.encode(), flags, "\\"
+
+
+def str_contains(col, pattern, literal: bool = False, strict: bool = True, location: int = HOST):
+    """str.contains.  literal=True (or a per-row pattern column with literal=True): bl_string_match(CONTAINS) on the bytes.
+    literal=False: the regex subset of regex_to_device runs on the device; any other regex raises B200Error status 4 so
+    the caller falls back (whatever `strict` says: the device does not tell an invalid regex from an unsupported one)."""
+    if literal or not isinstance(pattern, str):
+        if not literal and pattern is not None:
+            raise B200Error(4, "str_contains: a per-row or bytes regex pattern is not supported on the device")
+        return _str_match("contains", col, pattern, location=location)
+    kind, pat, flags, esc = regex_to_device(pattern)
+    return _str_match(kind, col, pat, flags, esc, location)
+
+
+def str_filter(col, mask, location: int = HOST):
+    """bl_string_filter: the rows of col whose mask bit is set (a null mask slot counts as false).  mask: a bool array,
+    (values, valid), Column or OutColumn.  -> list of bytes / None (host) or a DeviceStringColumn (device)."""
+    cc = _str_chunks(col)
+    m = _as_col(mask)
+    ms = m.struct()
+    out = BlStringColumn()
+    _check(lib().bl_string_filter(_str_array(cc), C.c_int32(len(cc)), C.byref(ms), C.c_int32(location), C.byref(out)))
+    return _string_out_to_list(out) if location == HOST else DeviceStringColumn(st=out)
+
+
 # ---------------------------------------------------------------------------------- operators
 def elementwise(op: str, lhs, rhs, location: int = HOST):
     l = _as_col(lhs) if not np.isscalar(lhs) else None

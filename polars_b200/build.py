@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_lib")
 SO = os.path.join(OUT_DIR, "libpolars_b200.so")
-SOURCES = ["runtime.cu", "elementwise.cu", "filter.cu", "gather.cu", "groupby.cu", "groupby_radix.cu", "groupby_exact.cu", "join.cu", "partition.cu", "sort.cu", "quantile.cu", "strings.cu", "string_rank.cu", "asof.cu", "ie_join.cu", "window.cu", "rolling.cu", "rolling_by.cu", "rolling_quantile.cu", "rank.cu", "top_k.cu", "unique.cu", "cabi.cu", "plugin.cu"]
+SOURCES = ["runtime.cu", "elementwise.cu", "filter.cu", "gather.cu", "groupby.cu", "groupby_radix.cu", "groupby_exact.cu", "join.cu", "partition.cu", "sort.cu", "quantile.cu", "strings.cu", "string_rank.cu", "asof.cu", "ie_join.cu", "window.cu", "rolling.cu", "rolling_by.cu", "rolling_quantile.cu", "rank.cu", "top_k.cu", "unique.cu", "string_match.cu", "cabi.cu", "plugin.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

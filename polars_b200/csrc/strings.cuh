@@ -16,6 +16,9 @@ struct DevStr {
 };
 
 DevStr import_string(const bl_string_column* chunks, int n_chunks);
+void export_string(const DevStr& s, int location, bl_string_column* out);
+// out[i] = s[idx[i]] (idx: UInt32; a null index, BL_IDX_NULL or a null row gives null); reads s.off() / s.bytes() only
+DevStr op_string_gather(const DevStr& s, const DevCol& idx);
 // code[row] = first row holding the same bytes (UInt32, validity = the input's); *n_distinct = distinct non-null values
 DevCol op_string_codes(const DevStr& s, int64_t* n_distinct);
 // dense lexicographic rank (UInt32, 1-based, validity = the input's; descending: the largest value is 1)
