@@ -89,6 +89,9 @@ void bl_shutdown(void);
 const char* bl_last_error(void);
 /* device facts for the host side: writes sm count, L2 bytes, total/free HBM bytes */
 bl_status bl_device_info(int32_t* sm_count, int64_t* l2_bytes, int64_t* hbm_total, int64_t* hbm_free);
+/* Returns the library's cached device blocks and its memory pool's unused memory to the driver, so that hbm_free counts
+   them and another allocator (PyTorch) can use them.  The next calls allocate afresh. */
+bl_status bl_release_cached(void);
 
 /* Deterministic aggregation (SURVEY.md §7(b)): on != 0 makes bl_groupby_agg / bl_groupby_agg_keys build the reference's
  * GroupsIdx and fold every group sequentially in row order with the reference's reducers (sequential Kahan float sums,

@@ -139,6 +139,12 @@ def device_info() -> dict:
     return {"sm_count": sm.value, "l2_bytes": l2.value, "hbm_total": tot.value, "hbm_free": free.value}
 
 
+def release_cached():
+    """Return the library's cached device blocks to the driver (bl_release_cached), as torch.cuda.empty_cache() does for
+    PyTorch's: afterwards device_info()["hbm_free"] counts them."""
+    _check(lib().bl_release_cached())
+
+
 def set_deterministic(on: bool = True):
     """Bit-stable group_by aggregation in the reference's own order (bl_set_deterministic)."""
     lib().bl_set_deterministic.restype = None

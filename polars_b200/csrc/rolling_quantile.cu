@@ -258,10 +258,13 @@ static WMatrix wm_build(const DevCol& v, const uint32_t* inv) {
     w.dtype = rolling_quantile_dtype(v.dtype);
     while ((int64_t(1) << w.L) < n) w.L++;
     w.level_words = (n / BV_TILE + 1) * (BV_TILE / BV_BITS) * 8;
-    DevPtr A = dev_alloc((size_t)n * 4);
-    w.V = dev_alloc((size_t)n * dtype_size(w.dtype));
+    DevPtr A;
     {
-        const DevCol sorted = op_arg_sort({v}, {BL_SORT_NULLS_LAST}, -1);      // its scratch is freed on return
+        // A and V are allocated after the sort, whose scratch is freed on return: the peak is the sort's plus the input,
+        // which keeps a column past 2^31 rows within one 80 GB device
+        const DevCol sorted = op_arg_sort({v}, {BL_SORT_NULLS_LAST}, -1);
+        A = dev_alloc((size_t)n * 4);
+        w.V = dev_alloc((size_t)n * dtype_size(w.dtype));
         const uint32_t* s = as<uint32_t>(sorted.values);
         switch (v.dtype) {
             case BL_INT8: launch_ranks<int8_t, double>(v, s, inv, as<uint32_t>(A), w.V->p); break;

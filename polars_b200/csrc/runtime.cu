@@ -381,6 +381,15 @@ bl_status bl_device_info(int32_t* sm_count, int64_t* l2_bytes, int64_t* hbm_tota
     if (hbm_free) *hbm_free = (int64_t)f;
     BL_CATCH
 }
+bl_status bl_release_cached(void) {
+    BL_TRY
+    Context& c = ctx();
+    { std::lock_guard<std::mutex> lk(g_init_mu); dev_cache_release_all(); }
+    cudaMemPool_t pool;
+    PLB_CUDA(cudaDeviceGetDefaultMemPool(&pool, c.device));
+    PLB_CUDA(cudaMemPoolTrimTo(pool, 0));
+    BL_CATCH
+}
 bl_status bl_alloc_pinned(size_t bytes, void** out) {
     BL_TRY
     PLB_REQUIRE(out, BL_ERR_INVALID, "null out");
